@@ -31,6 +31,7 @@ C2_WORKLOAD = ("C2: DeterministicPlannerAgent (OPD) plan() on HighwayLite (highw
 N_ACTIONS = 5
 STATE_BYTES = 136 * 4
 NODE_BYTES = 5 * 4 + 3 * 8          # parent, first_child, depth, count, meta + reward, lower, upper
+HBM_PEAK_GBS, HBM_PEAK_SOURCE = 3350.0, "data sheet (H100 SXM, 700 W)"    # roofline denominator, not a measurement
 
 
 def bench_config(a):
@@ -38,16 +39,19 @@ def bench_config(a):
     return {"workload": C2_WORKLOAD % (a.budget, a.gamma), "budget": a.budget, "gamma": a.gamma,
             "env": "HighwayLite", "n_actions": N_ACTIONS, "expansions_per_plan": a.budget // N_ACTIONS,
             "unit_of_work": "DeterministicNode.expand() calls (deterministic.py:28-43), strict best-first per tree",
-            "l2": "GPU arm: thousands of independent decisions per step, tree arenas >> 126 MB L2 (no flush needed)"}
+            "l2": "GPU arm: thousands of independent decisions per step, tree arenas >> 50 MB L2 (no flush needed)"}
 
 
 def parse():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=5)
+    ap.add_argument("--steps", type=int, default=5, help="timed steps (>= 1)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
-    ap.add_argument("--trees", type=int, default=0, help="decisions per GPU per step (default 128 per SM, capped by free HBM)")
+    ap.add_argument("--trees", type=int, default=0,
+                    help="decisions per GPU per step (default 128 per SM, capped by the GPU's memory size)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the timed path computed in its last step to DIR/<name>.npy")
     ap.add_argument("--budget", type=int, default=BUDGET)
     ap.add_argument("--gamma", type=float, default=GAMMA)
     ap.add_argument("--keys-in-smem", type=int, default=0)
@@ -57,7 +61,10 @@ def parse():
     ap.add_argument("--ref-time-box", type=float, default=420.0, help="--impl reference: stop after this many seconds")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--headline-only", action="store_true", help="skip the auxiliary paths (VI C4, MCTS C3, one-decision latency)")
-    return ap.parse_args()
+    a = ap.parse_args()
+    if a.steps < 1:
+        ap.error("--steps must be at least 1")
+    return a
 
 
 # ----------------------------------------------------------------------------
@@ -373,15 +380,23 @@ def run_b200(a):
     lib = _lib.load()
     sms = torch.cuda.get_device_properties(dev).multi_processor_count
     n_exp = a.budget // N_ACTIONS
+    trees_limited_by_free_memory = False
     if a.trees:
         trees = a.trees
     else:
         # default batch: 128 decisions per SM (more work in flight = better overlap of the trees' phases),
-        # capped so that the tree arena (scene + node record + frontier key per node) takes <= 65 % of the free HBM
+        # capped so that the tree arena (scene + node record + frontier key per node) takes <= 65 % of the GPU's
+        # memory (64 per SM on an 80 GB H100).  It depends on the device alone, so that the same arguments give
+        # the same inputs from run to run; only when other processes hold the memory it needs is it made smaller.
         per_tree = (1 + n_exp * N_ACTIONS) * (STATE_BYTES + NODE_BYTES + 8) + 16 * 1024
-        free, _ = torch.cuda.mem_get_info(dev)
-        trees = min(128 * sms, int(0.65 * free / per_tree))
+        free, total = torch.cuda.mem_get_info(dev)
+        trees = min(128 * sms, int(0.65 * total / per_tree))
         trees = max(8 * sms, trees // (8 * sms) * (8 * sms))
+        if trees * per_tree > 0.9 * free:
+            trees_limited_by_free_memory = True
+            trees = max(8 * sms, int(0.65 * free / per_tree) // (8 * sms) * (8 * sms))
+            print("bench.py: only %.1f GB free on the GPU, batch reduced to %d decisions" % (free / 1e9, trees),
+                  file=sys.stderr)
 
     eng = OPDEngine(_lib.ENV_HIGHWAY, trees, N_ACTIONS, a.budget, a.gamma, keys_in_smem=bool(a.keys_in_smem),
                     device=dev, kernel=a.kernel)
@@ -433,6 +448,8 @@ def run_b200(a):
     res = eng.result.cpu().numpy()
     assert (res[:, 0] > n_exp).all() and (res[:, 4] == 0).all()
     mean_children = float((res[:, 0] - 1).mean() / n_exp)
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, eng, res)
     # ---- e2e: the host-buffer C ABI (b2_opd_create / b2_opd_plan_host): pinned host scenes -> H2D -> search
     #      -> D2H of plans and per-tree results, synchronous, every step ----
     import ctypes
@@ -470,38 +487,12 @@ def run_b200(a):
     bytes_per_exp = STATE_BYTES * (1.0 + mean_children) + mean_children * (NODE_BYTES + 8 + 20) + 24
     launch_ms = ms / a.steps
     achieved = trees * n_exp * bytes_per_exp / (launch_ms * 1e-3) / 1e9
-    peak, peak_src = 6650.0, "fallback"
+    peak, peak_src = HBM_PEAK_GBS, HBM_PEAK_SOURCE
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             peak, peak_src = float(json.load(f)["hbm_gbs"]), "measured"
     except Exception:
         pass
-    traffic = None
-    try:
-        with open(os.path.join(ROOT, "profiles", "opd_highway_traffic.json")) as f:
-            tr = json.load(f)
-        if tr.get("trees") == trees and tr.get("budget") == a.budget:
-            traffic = tr["dram_bytes_per_launch"]
-    except Exception:
-        pass
-
-    ncu = None      # static evidence from the committed ncu capture of this kernel (not measured in this run)
-    for name in ("r02d_opd_multi_ncu_summary.json", "r02b_opd_multi_ncu_summary.json", "r01_opd_highway_multi_ncu_summary.json"):
-        try:
-            with open(os.path.join(ROOT, "profiles", name)) as f:
-                summ = json.load(f)
-            summ = summ.get("opd_highway_multi_kernel", summ)      # newer summaries are keyed by kernel name
-            inst = float(summ["smsp__inst_executed.sum"][0]) if "smsp__inst_executed.sum" in summ else None
-            ncu = {"source": "profiles/" + name,
-                   "ipc_per_sm": float(summ["sm__inst_executed.avg.per_cycle_elapsed"][0]),
-                   "issue_slots_busy_pct": float(summ["smsp__issue_active.avg.pct_of_peak_sustained_active"][0]),
-                   "alu_pipe_pct": float(summ["sm__inst_executed_pipe_alu.avg.pct_of_peak_sustained_active"][0]),
-                   "fma_pipe_pct": float(summ["sm__inst_executed_pipe_fma.avg.pct_of_peak_sustained_active"][0]),
-                   "dram_pct": float(summ["gpu__dram_throughput.avg.pct_of_peak_sustained_elapsed"][0]),
-                   "warp_instructions_in_capture": inst}
-            break
-        except Exception:
-            continue
     out = {
         "metric": "OPD leaf-expansions/sec on highway-v0 (HighwayLite)", "value": value, "unit": "expansions/s",
         "n_gpus": world, "steps": a.steps, "warmup": max(a.warmup, 3), "ms_per_step": ms / a.steps,
@@ -509,10 +500,11 @@ def run_b200(a):
         "config": bench_config(a),
         "run_config": {"trees_per_gpu": trees, "expansions_per_tree": n_exp,
                        "mean_children_per_expansion": mean_children, "child_nodes_per_s": value * mean_children,
-                       "l2": "working set %.1f GB per step >> 126 MB L2 (no flush needed)"
+                       "l2": "working set %.1f GB per step >> 50 MB L2 (no flush needed)"
                              % (trees * capacity * (STATE_BYTES + NODE_BYTES) / 1e9),
                        "parallelism": "trees sharded over %d GPU(s), no data-path collective" % world,
-                       "keys_in_smem": bool(a.keys_in_smem)},
+                       "keys_in_smem": bool(a.keys_in_smem),
+                       "trees_limited_by_free_memory": trees_limited_by_free_memory},
         "e2e": {"value": e2e_value, "unit": "expansions/s", "h2d_bytes_per_step": int(trees * STATE_BYTES),
                 "d2h_bytes_per_step": int(plan_host.numel() + res_host.numel() * 4), "ms_per_step": ms_e2e / a.steps,
                 "path": "b2_opd_plan_host (C ABI, host buffers, synchronous); wall clock over the steps, max over ranks"},
@@ -520,10 +512,10 @@ def run_b200(a):
         "per_rank": headline_per_rank,
         "clocks": clocks,
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                     "traffic": traffic, "peak_source": peak_src, "kernel": "opd_highway_multi_kernel",
-                     "bytes_per_expansion": bytes_per_exp, "limiter": "instruction issue (see ncu)", "ncu": ncu,
+                     "peak_source": peak_src, "kernel": "opd_highway_multi_kernel",
+                     "bytes_per_expansion": bytes_per_exp, "limiter": "instruction issue",
                      "note": "latency/FP32-issue bound by construction (15 dependent sub-steps per child); "
-                             "HBM fraction reported as the contract asks, see DESIGN.md section 4"},
+                             "the HBM fraction shows how far the kernel is from the memory bound, see DESIGN.md section 4"},
     }
     if not a.headline_only:
         try:
@@ -546,6 +538,47 @@ def run_b200(a):
         emit(out)
     if world > 1:
         dist.destroy_process_group()
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+OPD_RESULT_WORDS_WRITTEN = 7        # b2_opd_plan fills result words 0..6 of every tree; the rest are not written
+
+
+def dump_outputs(out_dir, eng, res, n_sample=8):
+    """What the last timed step computed, as a caller of OPDEngine receives it, in float64, at most 64 MB in all:
+    - per tree (every tree, or a fixed, seeded sample of trees when that would exceed 16 MB; `trees.npy` lists
+      them): the result words the kernel writes, the device part of the plan (-1 past its length), the root bounds;
+    - every node of a fixed, seeded sample of `n_sample` trees (0 past the tree's last node), cut to the first nodes
+      of each tree when that would exceed 32 MB.
+    About 16 MB at the default batch."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    rng = np.random.default_rng(0)
+    width = max(int(res[:, 5].max()), 1)
+    row_bytes = 8 * (OPD_RESULT_WORDS_WRITTEN + width + 2)
+    n_rows = min(eng.n_trees, (DUMP_LIMIT_BYTES // 4) // row_bytes)
+    rows = np.arange(eng.n_trees) if n_rows == eng.n_trees else np.sort(rng.choice(eng.n_trees, n_rows, replace=False))
+    rows_dev = torch.as_tensor(rows, device=eng.device)
+    plan_len = res[rows, 5]
+    plan = eng.plan_buf.index_select(0, rows_dev)[:, :width].cpu().numpy().astype(np.float64)
+    plan[np.arange(width)[None, :] >= plan_len[:, None]] = -1
+    arrays = {"trees": rows.astype(np.float64), "result": res[rows, :OPD_RESULT_WORDS_WRITTEN].astype(np.float64),
+              "plan": plan, "root_lower": eng.lower[:, 0].index_select(0, rows_dev).cpu().numpy(),
+              "root_upper": eng.upper[:, 0].index_select(0, rows_dev).cpu().numpy()}
+    fields = ("parent", "first_child", "depth", "count", "meta", "reward", "lower", "upper")
+    sample = np.sort(rng.choice(eng.n_trees, min(n_sample, eng.n_trees), replace=False))
+    n_nodes = min(eng.capacity, (DUMP_LIMIT_BYTES // 2) // (8 * len(fields) * len(sample)))
+    idx = torch.as_tensor(sample, device=eng.device)
+    beyond = np.arange(n_nodes)[None, :] >= res[sample, 0][:, None]
+    arrays["sample_trees"] = sample.astype(np.float64)
+    for name in fields:
+        x = getattr(eng, name).index_select(0, idx)[:, :n_nodes].cpu().numpy().astype(np.float64)
+        x[beyond] = 0
+        arrays["sample_" + name] = x
+    assert sum(x.nbytes for x in arrays.values()) <= DUMP_LIMIT_BYTES
+    for name, x in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), x)
 
 
 def other_paths(a, dev, world, rank):
@@ -587,7 +620,7 @@ def other_paths(a, dev, world, rank):
             best = ms if best is None else min(best, ms)
         return best
 
-    peak = 6650.0
+    peak = HBM_PEAK_GBS
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             peak = float(json.load(f)["hbm_gbs"])
@@ -619,7 +652,7 @@ def other_paths(a, dev, world, rank):
             full = timed_ms(lambda: eng.solve(sweeps))
             comp, nccl_full, p2p_full, p2p_err = full, None, None, None
         algo = float(S * A * B * 20 + S * A * 24 + S * 9)            # whole MDP, bytes per sweep (SURVEY 8d + Q_old)
-        # cold-L2 variant on one GPU: alternate between two table sets (2 x 0.8 GB >> 126 MB L2)
+        # cold-L2 variant on one GPU: alternate between two table sets (2 x 0.8 GB >> 50 MB L2)
         cold = None
         if world == 1:
             P2, N2, R2, term2 = garnet_slab(S, A, B, 0, S, seed=1, device=dev)
@@ -735,7 +768,6 @@ def other_paths(a, dev, world, rank):
         out["mcts_c3_wavefront"] = {
             "workload": "C3: MCTS on HighwayLite, 4096 episodes x horizon 20, ONE tree, waves of `width` episodes "
                         "(b2_mcts_plan_wave; specification oracle/planners.py::mcts_plan_wavefront, bit-exact)",
-            "strict_reference_order_ms": "2340 (one sequential chain of 81 920 env steps; profiles/r01_misc_measurements.json)",
             "rows": rows}
         torch.cuda.empty_cache()
     except Exception as ex:

@@ -15,7 +15,7 @@ sys.path.insert(0, ROOT)
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--trees", type=int, default=9472)
+    ap.add_argument("--trees", type=int, default=0, help="decisions per launch (default 64 per SM)")
     ap.add_argument("--episodes", type=int, default=256, help="C3 asks for 4096; 256 keeps the default run short")
     ap.add_argument("--horizon", type=int, default=20)
     ap.add_argument("--steps", type=int, default=1)
@@ -25,6 +25,8 @@ def main():
     from rl_agents_b200.engine.mcts import MCTSEngine, pcg64_words
     from rl_agents_b200.envs.highway_lite import make_scene
     dev = torch.device("cuda", 0)
+    if not a.trees:
+        a.trees = 64 * torch.cuda.get_device_properties(dev).multi_processor_count
     eng = MCTSEngine(_lib.ENV_HIGHWAY, a.trees, 5, a.episodes, a.horizon, 0.8, 10.0, device=dev)
     scenes = torch.from_numpy(np.stack([make_scene(i) for i in range(a.trees)])).to(dev)
     gens = [np.random.Generator(np.random.PCG64(np.random.SeedSequence(i))) for i in range(a.trees)]

@@ -43,7 +43,7 @@ def main():
         eng.plan(scene, 0)
         plan, res = eng.finish()
         waves = int(res[3])
-        prof = res[4:8].astype(float) * 256 / 1965.0 / waves
+        prof = res[4:8].astype(float) * 256 / (torch.cuda.get_device_properties(0).clock_rate / 1e3) / waves
         counts, values = eng.root_statistics()
         rows.append({"mode": "wavefront", "width": width, "ms": ms, "episodes_per_s": E / (ms * 1e-3),
                      "env_steps": int(res[2]), "env_steps_per_s": int(res[2]) / (ms * 1e-3), "waves": waves,

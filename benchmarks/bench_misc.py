@@ -72,13 +72,13 @@ def main():
         out["opd_highway_b1e6_sharded_subtrees"] = d["n_subtrees"]
 
     # --- batches ---
-    n = 148 * 256
+    n = torch.cuda.get_device_properties(dev).multi_processor_count * 256
     roots = torch.randint(0, 100, (n,), dtype=torch.int32, device=dev)
     eng = OPDEngine(_lib.ENV_FINITE, n, 5, 10000, 0.9, mdp=mdp)
     ms = timed(lambda: eng.plan(roots), reps=3)
     out["opd_finite_b10000_batch"] = {"trees": n, "ms": ms, "expansions_per_s": n * 2000 / (ms * 1e-3)}
     ub = {"type": "kullback-leibler", "time": "global", "threshold": "2*np.log(time)"}
-    n = 9472
+    n = torch.cuda.get_device_properties(dev).multi_processor_count * 64
     scenes = torch.from_numpy(np.stack([make_scene(i) for i in range(n)])).to(dev)
     oeng = OLOPEngine(_lib.ENV_HIGHWAY, n, 5, 72, 6, 0.7, ub, "uniform")      # budget 500, gamma 0.7 (shipped KL-OLOP config)
     words = np.stack([pcg64_words(np.random.Generator(np.random.PCG64(i))) for i in range(n)])

@@ -21,7 +21,7 @@ def main():
     ap.add_argument("--seeds", type=int, default=2)
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--strict", type=int, default=1)
-    ap.add_argument("--sm-mhz", type=float, default=1965.0)
+    ap.add_argument("--sm-mhz", type=float, default=0.0, help="SM clock for the clock64 profile (default: the device's)")
     a = ap.parse_args()
     import numpy as np
     import torch
@@ -29,6 +29,7 @@ def main():
     from rl_agents_b200.engine.opd import OPDEngine, OPDSpeculativeEngine
     from rl_agents_b200.envs.highway_lite import make_scene
     scenes = [torch.tensor(make_scene(s), dtype=torch.int32, device="cuda") for s in range(a.seeds)]
+    sm_mhz = a.sm_mhz or torch.cuda.get_device_properties(0).clock_rate / 1e3
 
     def med_ms(fn):
         fn()
@@ -61,7 +62,7 @@ def main():
                 waves = int(res[7])
                 names = ["commit", "select", "sort_worklist", "barrier_after_select", "simulate", "barrier_after_simulate",
                          "bottom_up_plan"]
-                per_wave = {n: float(res[8 + i]) * 256.0 / a.sm_mhz / max(waves, 1) for i, n in enumerate(names)}
+                per_wave = {n: float(res[8 + i]) * 256.0 / sm_mhz / max(waves, 1) for i, n in enumerate(names)}
                 rows.append({"budget": budget, "gamma": gamma, "kernel": "b2_opd_plan_spec", "candidates": width, "ms": ms,
                              "expansions_per_s": n_exp / (ms * 1e-3), "waves": waves,
                              "commits_per_wave": n_exp / float(max(waves, 1)), "max_depth": int(res[2]),

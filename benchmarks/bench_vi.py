@@ -78,7 +78,8 @@ def main():
     assert int(eng.viol.min().item()) > 0               # every sweep did its work
     per_sweep_ms = ms / a.sweeps
     slab_bytes = eng.bytes_per_sweep()
-    peak = 6650.0
+    from bench import HBM_PEAK_GBS
+    peak = HBM_PEAK_GBS
     try:
         peak = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"])
     except Exception:

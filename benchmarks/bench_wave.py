@@ -14,6 +14,10 @@ from rl_agents_b200.engine.opd import OPDEngine, OPDWaveEngine    # noqa: E402
 from rl_agents_b200.envs.highway_lite import make_scene          # noqa: E402
 
 
+def sm_mhz():
+    return torch.cuda.get_device_properties(0).clock_rate / 1e3
+
+
 def time_ms(fn, reps):
     fn()
     torch.cuda.synchronize()
@@ -69,7 +73,7 @@ def main():
                 gaps.append(strict_lower[i] - float(eng.lower[0, 0].item()))
         names = ["stage", "bisect", "compact_layout", "barrier_after_select", "simulate", "barrier_after_simulate", "finish"]
         prof = res[0, 8:16].astype(float)
-        row["prof_us_per_wave"] = {n: round(float(prof[i]) * 256 / 1965.0 / waves[-1], 2) for i, n in enumerate(names)}
+        row["prof_us_per_wave"] = {n: round(float(prof[i]) * 256 / sm_mhz() / waves[-1], 2) for i, n in enumerate(names)}
         row["bisection_steps_per_wave"] = float(prof[7]) / waves[-1]
         row["waves"] = float(np.mean(waves))
         row["us_per_wave"] = 1e3 * float(ms) / row["waves"]

@@ -1,5 +1,5 @@
 /*
- * b2_planner.h -- C ABI of libb2planner.so, the B200 (sm_100a) planning engine
+ * b2_planner.h -- C ABI of libb2planner.so, the H100 (sm_90a) planning engine
  * behind the rl-agents plugin surface.
  *
  * Every entry point replaces the inner loop of one reference method (cited as

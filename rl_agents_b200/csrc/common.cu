@@ -13,7 +13,7 @@ void set_error(const char* fmt, ...) {
 }
 
 int sm_count() {
-    int dev = 0, n = 148;
+    int dev = 0, n = 132;
     if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
     return n;
 }

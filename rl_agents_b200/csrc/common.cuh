@@ -1,4 +1,4 @@
-// Shared host/device helpers of libb2planner (sm_100a only).
+// Shared host/device helpers of libb2planner (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

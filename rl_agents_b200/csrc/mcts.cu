@@ -75,7 +75,7 @@ struct HighwayEnv {
 
 // --------------------------------------------------------------- kernel ---
 #ifndef B2_MCTS_MIN_BLOCKS
-#define B2_MCTS_MIN_BLOCKS 8   // 64 registers, 32 warps/SM: measured best (6.5M vs 5.8M episodes/s at 4)
+#define B2_MCTS_MIN_BLOCKS 8   // 64 registers, 32 warps/SM
 #endif
 template <class Env>
 __global__ void __launch_bounds__(128, B2_MCTS_MIN_BLOCKS) mcts_kernel(MctsArgs a) {

@@ -1,7 +1,7 @@
 // Wavefront MCTS: ONE decision searched by the whole GPU (b2_mcts_plan_wave).
 //
 // The reference's MCTS.plan (mcts.py:179-184) runs its episodes one after the other on one sequential RNG
-// stream: 4096 episodes x horizon 20 is a chain of 81 920 dependent env transitions (2.3 s on a B200).  The
+// stream: 4096 episodes x horizon 20 is a chain of 81 920 dependent env transitions.  The
 // wavefront keeps the reference's episode -- selection (:141-149), expansion (:151-154), rollout (:160-177),
 // backup (:257-265), recommendation (:212-218) -- and runs the episodes in waves of `width`:
 //   select (CTA 0)   all selections of the wave, level by level.  A node's arrivals are a contiguous, episode-

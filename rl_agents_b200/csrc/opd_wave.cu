@@ -1,8 +1,8 @@
 // Wavefront OPD: ONE decision searched by the whole GPU (b2_opd_plan_wave).
 //
 // The reference's OptimisticDeterministicPlanner.run (deterministic.py:106-114) expands one leaf per
-// iteration -- a chain of `budget / n_actions` dependent env transitions (28 us each on a B200 for
-// HighwayLite).  The wavefront expands, per wave, the k = min(width, expansions left, frontier size) best
+// iteration -- a chain of `budget / n_actions` dependent env transitions.
+// The wavefront expands, per wave, the k = min(width, expansions left, frontier size) best
 // leaves in the reference's own arg-max order (value_upper descending, node id ascending, :110), in
 // increasing node-id order, and simulates all their children at once on every SM.  width = 1 is the
 // reference's algorithm; the specification for any width is oracle/planners.py::opd_plan_wavefront, and the

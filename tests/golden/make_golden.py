@@ -428,8 +428,37 @@ def highway_vi():
     print("highway VI done:", len(out["cases"]), "cases")
 
 
+def host():
+    """The host side of the plugin surface -> tests/golden/golden_host.json: the method names of the reference's
+    AbstractAgent, the completed configs of its DeterministicPlannerAgent / MCTSAgent, and what its
+    AbstractTreeSearchAgent does under every receding horizon when driven by a scripted planner
+    (tests/test_host.py drives the drop-in agent shell with the same script)."""
+    import inspect
+    from rl_agents.agents.common.abstract import AbstractAgent
+    from rl_agents.agents.tree_search.abstract import AbstractTreeSearchAgent
+    from tests.test_host import run_scripted_agent
+    from tests.util import load_mdps
+    out = {"abstract_agent_methods": sorted(n for n, _ in inspect.getmembers(AbstractAgent, inspect.isfunction)
+                                            if not n.startswith("_")),
+           "configs": {}, "receding_horizon": {}}
+    m = load_mdps()
+    env = envs.FiniteMDPLite(m["large1_T"], m["large1_R"], m["large1_term"])
+    for name, cls, cfg in [("DeterministicPlannerAgent", ref_det.DeterministicPlannerAgent, {"budget": 75}),
+                           ("MCTSAgent", ref_mcts.MCTSAgent, {"budget": 400, "gamma": 0.9})]:
+        out["configs"][name] = {"config": cfg, "completed": dict(cls(env, dict(cfg)).config)}
+    for receding_horizon in (1, 2, 3, 5):
+        outs, log, config = run_scripted_agent(AbstractTreeSearchAgent, receding_horizon)
+        out["receding_horizon"][str(receding_horizon)] = {"plans": outs, "log": log, "config": config}
+    with open(os.path.join(HERE, "golden_host.json"), "w") as f:
+        json.dump(out, f)
+    print("host done")
+
+
 if __name__ == "__main__":
     if "--only-highway-vi" in sys.argv:
         highway_vi()
+    elif "--only-host" in sys.argv:
+        host()
     else:
         main()
+        host()

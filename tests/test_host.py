@@ -2,6 +2,7 @@
 spec constants in the CUDA header equal the oracle's fp32 values, and the host
 side of the plugin surface (config merge, defaults, allocation, env hand-off,
 the reference's own agent_factory) behaves like the reference's."""
+import json
 import os
 import re
 
@@ -9,7 +10,6 @@ import numpy as np
 import pytest
 
 from oracle import envs as oenvs
-from oracle import ref_loader
 from tests.util import load_golden, load_mdps
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -88,25 +88,22 @@ def test_agent_defaults_match_reference_defaults():
         MCTSAgent(env, {"rollout_policy": {"type": "nope"}})
 
 
-@pytest.mark.skipif(not ref_loader.reference_available(), reason="reference tree not present")
-def test_reference_defaults_and_factory_accept_the_drop_in():
-    """The reference's own loader (factory.py:12-27) builds our agents from a
-    `__class__` string, and their completed configs equal the reference agents'."""
-    ref_loader.load_reference()
-    from rl_agents.agents.common.abstract import AbstractAgent as RefAbstractAgent
-    from rl_agents.agents.common.factory import agent_factory
-    from rl_agents.agents.tree_search.deterministic import DeterministicPlannerAgent as RefOPD
-    from rl_agents.agents.tree_search.mcts import MCTSAgent as RefMCTS
+def test_drop_in_agents_have_the_reference_configs_and_interface():
+    """Our DeterministicPlannerAgent / MCTSAgent, built as the reference's agent_factory builds a class named by
+    `__class__` (factory.py:12-27: `Class(env, config)` with the `__class__` key left in), complete their configs to the
+    reference agents' and offer every method of the reference's AbstractAgent; both are recorded from the reference
+    in golden_host.json by tests/golden/make_golden.py."""
+    from rl_agents_b200.agents.tree_search.deterministic import DeterministicPlannerAgent
+    from rl_agents_b200.agents.tree_search.mcts import MCTSAgent
+    golden = load_golden("golden_host.json")
     env = oenvs.FiniteMDPLite(M["large1_T"], M["large1_R"], M["large1_term"])
-    for path, ref_cls, cfg in [
-            ("rl_agents_b200.agents.tree_search.deterministic.DeterministicPlannerAgent", RefOPD, {"budget": 75}),
-            ("rl_agents_b200.agents.tree_search.mcts.MCTSAgent", RefMCTS, {"budget": 400, "gamma": 0.9})]:
-        mine = agent_factory(env, dict(cfg, __class__="<class '%s'>" % path))
-        ref = ref_cls(env, dict(cfg))
-        theirs = dict(ref.config)
-        ours = {k: v for k, v in mine.config.items() if k != "__class__"}
+    for cls in (DeterministicPlannerAgent, MCTSAgent):
+        g = golden["configs"][cls.__name__]
+        mine = cls(env, dict(g["config"], __class__="<class '%s.%s'>" % (cls.__module__, cls.__name__)))
+        theirs = g["completed"]
+        ours = json.loads(json.dumps({k: v for k, v in mine.config.items() if k != "__class__"}))
         assert ours == theirs
-        assert isinstance(mine, RefAbstractAgent)
+        assert all(callable(getattr(mine, m, None)) for m in golden["abstract_agent_methods"])
         assert mine.config.get("gamma", 1) == theirs["gamma"]     # evaluation.py:327 reads it
 
 
@@ -142,15 +139,21 @@ def test_finite_env_steps_like_the_oracle_env():
         assert a.step(act) == b.step(act)
 
 
-@pytest.mark.skipif(not ref_loader.reference_available(), reason="reference tree not present")
 @pytest.mark.parametrize("receding_horizon", [1, 2, 3, 5])
 def test_receding_horizon_schedule_matches_the_reference_agent(receding_horizon):
     """The agent shell (own implementation) against the reference's AbstractTreeSearchAgent driven by the
-    same scripted planner: identical plan() outputs, planner calls and step_tree arguments."""
-    ref_loader.load_reference()
-    from rl_agents.agents.tree_search.abstract import AbstractTreeSearchAgent as RefAgent
+    same scripted planner (golden_host.json, recorded from the reference by tests/golden/make_golden.py):
+    identical plan() outputs, planner calls and step_tree arguments."""
     from rl_agents_b200.agents.tree_search.abstract import AbstractTreeSearchAgent as OurAgent
+    ours = json.loads(json.dumps(run_scripted_agent(OurAgent, receding_horizon)))
+    ref = load_golden("golden_host.json")["receding_horizon"][str(receding_horizon)]
+    assert ours[0] == ref["plans"] and ours[1] == ref["log"]
+    assert ours[2] == ref["config"]
 
+
+def run_scripted_agent(agent_cls, receding_horizon):
+    """Drive a subclass of `agent_cls` (an AbstractTreeSearchAgent) with a scripted planner over 25 decisions and
+    a reset: returns (plan() outputs, the planner's call log, the completed config)."""
     lengths = [4, 1, 3, 2, 6, 1, 1, 5, 3]
 
     class Scripted(object):
@@ -175,20 +178,15 @@ def test_receding_horizon_schedule_matches_the_reference_agent(receding_horizon)
     class Env(object):
         unwrapped = property(lambda self: self)
 
-    def run(cls):
-        class A(cls):
-            PLANNER_TYPE = Scripted
-        a = A(Env(), {"receding_horizon": receding_horizon})
-        outs = []
-        for t in range(25):
-            if t == 13:
-                a.reset()
-            outs.append(list(a.plan(t)))
-        return outs, a.planner.log, a.config
-
-    ours, ref = run(OurAgent), run(RefAgent)
-    assert ours[0] == ref[0] and ours[1] == ref[1]
-    assert ours[2] == ref[2]
+    class A(agent_cls):
+        PLANNER_TYPE = Scripted
+    a = A(Env(), {"receding_horizon": receding_horizon})
+    outs = []
+    for t in range(25):
+        if t == 13:
+            a.reset()
+        outs.append(list(a.plan(t)))
+    return outs, a.planner.log, a.config
 
 
 def test_preprocess_env_applies_methods_in_sequence():
