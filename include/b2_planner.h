@@ -487,6 +487,52 @@ typedef struct b2_olop_tree {
 int b2_olop_plan(const b2_olop_config* cfg, const int32_t* root_states, const b2_olop_tree* tree,
                  uint64_t* rng, int8_t* plan, int32_t* result, void* stream);
 
+/* ------------------------------------------------------------------------
+ * MDP-GapE -- rl_agents/agents/tree_search/mdp_gape.py (KL upper bound; deterministic env models, so only
+ * one next state per chance node is ever observed)
+ * ---------------------------------------------------------------------- */
+typedef struct b2_mdp_gape_config {
+    int32_t env_kind;
+    int32_t n_trees;
+    int32_t n_actions;
+    int32_t episodes;        /* config["episodes"]; the stopping rule runs at most episodes + 2 (:94-110) */
+    int32_t horizon;         /* config["horizon"]                            */
+    int32_t node_capacity;   /* per tree, >= 1 + (episodes+2)*horizon*(n_actions+max_next_states) */
+    int32_t max_next_states; /* config["max_next_states_count"]: placeholders per chance node (:267-270) */
+    int32_t continuation;    /* 0 "zeros", 1 "uniform" (:194-196)              */
+    double gamma;
+    double accuracy;         /* stopping rule: challenger.upper - best.lower < accuracy (:101) */
+    const double* thresholds;            /* [episodes+3] eval(upper_bound.threshold) by count (:200-212) */
+    const double* transition_thresholds; /* [episodes+3] eval(upper_bound.transition_threshold) by count (:307-313) */
+    const double* init_upper;/* [horizon+1] (1 - gamma**(H-d)) / (1 - gamma) by depth d (:145-147) */
+    b2_finite_mdp mdp;
+} b2_mdp_gape_config;
+
+/* One arena for decision and chance nodes; node id = creation order (placeholders in index order, chance nodes in
+ * available-action order).  The children of a chance node are its placeholders fc .. fc+K-1; the observed one is
+ * fc, which the reference moves to the end of its child order. */
+typedef struct b2_mdp_gape_tree {
+    int32_t* parent;
+    int32_t* first_child;
+    int32_t* count;
+    int32_t* meta;           /* label | n_children << 8 | done << 16 | kind << 17; label = action (chance node),
+                                placeholder index (decision node), 0xff (root); kind 0 decision, 1 chance */
+    double* cumulative;      /* DecisionNode.cumulative_reward                 */
+    double* mu_ucb;          /* KL upper / lower bound of the mean reward      */
+    double* mu_lcb;
+    double* upper;           /* value_upper                                    */
+    double* lower;           /* value_lower                                    */
+} b2_mdp_gape_tree;
+
+#define B2_MDP_GAPE_RESULT_WORDS 8
+/* per tree int32 result: [0] n_nodes [1] episodes run [2] error (1: reward outside [0,1], olop.py:133-134;
+ * 2: a single available action at the root -- max() of an empty list in the reference, :247) [3] recommended
+ * action [4] best [5] challenger (root children's node ids, UGapE :238-249) */
+
+/* MDPGapE.plan (:94-110); rng as in b2_mcts_plan; plan: int8 [n_trees], the recommended action (-1 on error). */
+int b2_mdp_gape_plan(const b2_mdp_gape_config* cfg, const int32_t* root_states, const b2_mdp_gape_tree* tree,
+                     uint64_t* rng, int8_t* plan, int32_t* result, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -19,6 +19,7 @@ VI_DETERMINISTIC, VI_STOCHASTIC, VI_SPARSE = 0, 1, 2
 OPD_RESULT_WORDS = 16
 MCTS_RESULT_WORDS = 8
 OLOP_RESULT_WORDS = 8
+MDP_GAPE_RESULT_WORDS = 8
 PCG64_STATE_WORDS = 6
 
 
@@ -121,6 +122,20 @@ class OLOPTree(ctypes.Structure):
     _fields_ = [(n, c_void_p) for n in ("parent", "first_child", "count", "meta", "cumulative", "mu_ucb", "upper")]
 
 
+class MDPGapEConfig(ctypes.Structure):
+    _fields_ = [("env_kind", c_int32), ("n_trees", c_int32), ("n_actions", c_int32), ("episodes", c_int32),
+                ("horizon", c_int32), ("node_capacity", c_int32), ("max_next_states", c_int32),
+                ("continuation", c_int32), ("gamma", c_double), ("accuracy", c_double), ("thresholds", c_void_p),
+                ("transition_thresholds", c_void_p), ("init_upper", c_void_p), ("mdp", FiniteMDP)]
+
+
+MDP_GAPE_TREE_FIELDS = ("parent", "first_child", "count", "meta", "cumulative", "mu_ucb", "mu_lcb", "upper", "lower")
+
+
+class MDPGapETree(ctypes.Structure):
+    _fields_ = [(n, c_void_p) for n in MDP_GAPE_TREE_FIELDS]
+
+
 EXPORTS = {
     "b2_last_error": (ctypes.c_char_p, []),
     "b2_version": (c_int, []),
@@ -166,6 +181,8 @@ EXPORTS = {
                                   c_void_p, c_void_p, c_void_p]),
     "b2_olop_plan": (c_int, [ctypes.POINTER(OLOPConfig), c_void_p, ctypes.POINTER(OLOPTree), c_void_p, c_void_p,
                              c_void_p, c_void_p]),
+    "b2_mdp_gape_plan": (c_int, [ctypes.POINTER(MDPGapEConfig), c_void_p, ctypes.POINTER(MDPGapETree), c_void_p,
+                                 c_void_p, c_void_p, c_void_p]),
 }
 
 _lib = None

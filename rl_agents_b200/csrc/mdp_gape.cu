@@ -1,0 +1,352 @@
+// MDP-GapE -- the plan() loop of rl_agents/agents/tree_search/mdp_gape.py for a BATCH of independent
+// decisions.  Strict episode order inside each tree; the planner's numpy PCG64 stream is consumed exactly as
+// the reference does (`np_random.randint(2**30)` per episode, :67; `randint(n_actions)` for the "uniform"
+// continuation, :195; `choice(indices)` for ties of random_argmax, abstract.py:296-311).  The KL bounds of a
+// decision node (utils.py:123-203, damped Newton on the Bernoulli KL, kl_bound.cuh -- the iteration OLOP uses) run
+// in-kernel in fp64.
+//
+// The tree alternates decision nodes (value bounds, KL statistics of the reward received on arrival) and chance
+// nodes (one per available action).  A chance node's children are max_next_states_count placeholders; the env
+// models here are deterministic, so only placeholder 0 is ever observed, and it is moved to the END of the
+// chance node's child order (mdp_gape.py:272-286) -- the order in which the backup sums.  Then
+// max_expectation_under_constraint (utils.py:292-342) sees a distribution with one positive element and needs
+// no Newton solve: it is restated operation by operation in gape_expectation().
+//
+// Same lane-group mapping as olop.cu: one tree per 16-lane group (HighwayLite, lane = vehicle slot) or per lane
+// (finite MDP).  Every lane of a group holds a copy of the tree's RNG and takes every selection decision
+// itself from the tree arrays; lane 0 writes the tree.  A tree whose stopping rule fired leaves its episode
+// loop; hw::step only synchronises the 16 lanes of one group, so the other trees of the warp carry on.
+#include "common.cuh"
+#include "highway_lite.cuh"
+#include "kl_bound.cuh"
+#include "pcg64.cuh"
+
+namespace b2 {
+namespace {
+
+constexpr int KIND_DECISION = 0, KIND_CHANCE = 1;
+constexpr int DONE_BIT = 1 << 16, KIND_SHIFT = 17;
+
+struct GapeArgs {
+    b2_mdp_gape_config cfg;
+    b2_mdp_gape_tree tree;
+    const int32_t* root_states;
+    uint64_t* rng;
+    int8_t* plan;
+    int32_t* result;
+};
+
+// ChanceNode.backup_to_root (mdp_gape.py:288-305) for one side: with f = u_next (upper) or -l_next (lower),
+// p = max_expectation_under_constraint(f, p_hat, c) and the bound is p @ (u_next | l_next).  Children in the
+// reference's dict order: the unobserved placeholders fc+1 .. fc+k-1, then the observed fc, whose p_hat is qp.
+__device__ double gape_expectation(const b2_mdp_gape_tree& tr, int64_t nb, int fc, int k, bool upper_side,
+                                   double gamma, double qp, double c) {
+    auto value = [&](int id) {
+        return upper_side ? tr.mu_ucb[nb + id] + gamma * tr.upper[nb + id] : tr.mu_lcb[nb + id] + gamma * tr.lower[nb + id];
+    };
+    const double fp = upper_side ? value(fc) : -value(fc);
+    double f_star = fp, f_zero_max = -INFINITY;
+    for (int i = 1; i < k; ++i) {
+        const double f = upper_side ? value(fc + i) : -value(fc + i);
+        f_star = f > f_star ? f : f_star;
+        f_zero_max = f > f_zero_max ? f : f_zero_max;
+    }
+    // utils.py:317-323: move the mass z = 1 - exp(theta(f*)) to the best unobserved entries when theta(f*) < 0,
+    // theta(l) = q_p @ log(l - f_p) + log(q_p @ (1 / (l - f_p))) - c (theta_func, :279-282)
+    double z = 0.0, d = 0.0;
+    bool moved = false;
+    if (f_star > fp) {
+        d = f_star - fp;
+        const double theta = qp * log(d) + log(qp * (1.0 / d)) - c;
+        if (theta < 0.0) {
+            moved = true;
+            z = 1.0 - exp(theta);
+        }
+    }
+    double p_obs = qp, share = 0.0;
+    if (moved) {
+        int n_max = 0;
+        for (int i = 1; i < k; ++i) n_max += (upper_side ? value(fc + i) : -value(fc + i)) == f_zero_max;
+        share = z / (double)n_max;
+        const double beta = (1.0 - z) / (qp * (1.0 / d));          // :335, lambda = f*
+        p_obs = beta != 0.0 ? (beta * qp) / d : 0.0;               // :336-341 (no observed entry reaches f*)
+    }
+    // p @ next in the dict order
+    double s = 0.0;
+    for (int i = 1; i < k; ++i) {
+        const double v = value(fc + i);
+        const double p = moved ? (((upper_side ? v : -v) == f_zero_max) ? 1.0 : 0.0) * share : 0.0;
+        s = s + p * v;
+    }
+    return s + p_obs * value(fc);
+}
+
+// best_arm_identification_selection (mdp_gape.py:228-249) on the children fc .. fc+n-1 (n >= 2): UGapE's best
+// (first minimum of the gap), challenger (first maximum of value_upper among the others) and the sampled arm
+// (the wider interval of the two, best on a tie).  Node ids.
+__device__ void bai(const b2_mdp_gape_tree& tr, int64_t nb, int fc, int n, int& sel, int& best, int& challenger) {
+    int bi = 0;
+    double best_gap = 0.0;
+    for (int i = 0; i < n; ++i) {
+        double g = -INFINITY;
+        const double lo = tr.lower[nb + fc + i];
+        for (int j = 0; j < n; ++j) {
+            if (j == i) continue;
+            const double x = tr.upper[nb + fc + j] - lo;
+            if (x > g) g = x;
+        }
+        if (i == 0 || g < best_gap) { best_gap = g; bi = i; }
+    }
+    int ci = -1;
+    double cu = 0.0;
+    for (int j = 0; j < n; ++j) {
+        if (j == bi) continue;
+        const double u = tr.upper[nb + fc + j];
+        if (ci < 0 || u > cu) { ci = j; cu = u; }
+    }
+    best = fc + bi;
+    challenger = fc + ci;
+    const double wb = tr.upper[nb + best] - tr.lower[nb + best];
+    const double wc = tr.upper[nb + challenger] - tr.lower[nb + challenger];
+    sel = wc > wb ? challenger : best;
+}
+
+__device__ __forceinline__ void new_node(const b2_mdp_gape_tree& tr, int64_t nb, int id, int parent, int label,
+                                         int kind, double init_upper) {
+    tr.parent[nb + id] = parent; tr.first_child[nb + id] = -1; tr.count[nb + id] = 0;
+    tr.meta[nb + id] = label | (kind << KIND_SHIFT);
+    tr.cumulative[nb + id] = 0.0; tr.mu_ucb[nb + id] = 1.0; tr.mu_lcb[nb + id] = 0.0;   // KL (mdp_gape.py:139-143)
+    tr.upper[nb + id] = init_upper; tr.lower[nb + id] = 0.0;
+}
+
+struct GFiniteEnv {
+    static constexpr int GROUP = 1;
+    int s;
+    __device__ __forceinline__ void load_root(const GapeArgs& a, int tree, int li) { s = a.root_states[tree]; }
+    __device__ __forceinline__ int avail(const GapeArgs& a, unsigned gmask) const { return (1 << a.cfg.n_actions) - 1; }
+    __device__ __forceinline__ static int nth(int mask, int n) { return n; }
+    __device__ __forceinline__ double step(const GapeArgs& a, int action, int li, unsigned gmask, float* gs, bool& term) {
+        const b2_finite_mdp& m = a.cfg.mdp;
+        const double r = m.reward[(int64_t)s * m.n_actions + action];
+        term = m.terminal[s] != 0;        // done = terminal[state BEFORE the transition]
+        s = m.transition[(int64_t)s * m.n_actions + action];
+        return r;
+    }
+};
+
+struct GHighwayEnv {
+    static constexpr int GROUP = 16;
+    hw::Lane L;
+    int t, si;
+    __device__ __forceinline__ void load_root(const GapeArgs& a, int tree, int li) {
+        hw::load_state(a.root_states + (int64_t)tree * hw::WORDS, li, L, t, si);
+    }
+    __device__ __forceinline__ int avail(const GapeArgs& a, unsigned gmask) const {
+        return hw::avail_mask(__shfl_sync(gmask, L.y, 0, 16), si);
+    }
+    __device__ __forceinline__ static int nth(int mask, int n) { return hw::nth_action(mask, n); }
+    __device__ __forceinline__ double step(const GapeArgs& a, int action, int li, unsigned gmask, float* gs, bool& term) {
+        bool trunc;
+        return (double)hw::step(L, li, t, si, action, term, trunc, gmask, gs);
+    }
+};
+
+template <class Env>
+__global__ void __launch_bounds__(128, 8) mdp_gape_kernel(GapeArgs a) {
+    constexpr int G = Env::GROUP;
+    __shared__ float scratch[G == 16 ? 128 / 16 : 1][hw::SCRATCH_FLOATS];
+    const int gtid = blockIdx.x * 128 + threadIdx.x;
+    const int tree = gtid / G, li = gtid % G;
+    if (tree >= a.cfg.n_trees) return;              // whole lane groups: no live lane of a group leaves here
+    const bool writer = li == 0;
+    const int lane = threadIdx.x & 31;
+    const unsigned gmask = G == 1 ? (1u << lane) : (0xFFFFu << (lane & 16));
+    const int H = a.cfg.horizon, K = a.cfg.max_next_states;
+    const int64_t nb = (int64_t)tree * a.cfg.node_capacity;
+    const b2_mdp_gape_tree& tr = a.tree;
+    const double gamma = a.cfg.gamma;
+    float* gs = scratch[(threadIdx.x >> 4) % (128 / 16)];
+
+    Pcg64 rng;
+    rng.load(a.rng + (int64_t)tree * B2_PCG64_STATE_WORDS);
+    if (writer) new_node(tr, nb, 0, -1, 0xff, KIND_DECISION, a.cfg.init_upper[0]);    // DecisionNode(None)
+    __syncwarp(gmask);
+    int n_nodes = 1, error = 0, episode = 0, best = -1, challenger = -1;
+    bool done = false;
+
+    // expand a decision node (mdp_gape.py:162-170): one chance node per available action, env order
+    auto expand_decision = [&](int node, int amask, int depth) {
+        const int n = __popc(amask);
+        if (writer) {
+            for (int i = 0; i < n; ++i) new_node(tr, nb, n_nodes + i, node, Env::nth(amask, i), KIND_CHANCE,
+                                                  a.cfg.init_upper[depth]);
+            tr.first_child[nb + node] = n_nodes;
+            tr.meta[nb + node] = (tr.meta[nb + node] & ~0xff00) | (n << 8);
+        }
+        n_nodes += n;
+        __syncwarp(gmask);
+    };
+
+    while (!done) {                                  // MDPGapE.plan (:94-110)
+        Env env;
+        env.load_root(a, tree, li);                  // safe_deepcopy_env(state), :98
+        rng.integers(1u << 30);                      // state.seed(np_random.randint(2**30)), :67
+        if (tr.first_child[nb] < 0) expand_decision(0, env.avail(a, gmask), 0);
+        int node = 0;
+        for (int h = 0; h < H; ++h) {
+            const int amask = env.avail(a, gmask);
+            int fc = tr.first_child[nb + node];
+            // sampling_rule (:183-198)
+            int action;
+            if (node == 0) {
+                const int n = (tr.meta[nb] >> 8) & 0xff;
+                if (n < 2) { error = 2; break; }     // max() of an empty challenger list: ValueError
+                int sel;
+                bai(tr, nb, fc, n, sel, best, challenger);
+                action = tr.meta[nb + sel] & 0xff;
+            } else if (fc >= 0) {                    // random_argmax of the chance children's value_upper
+                const int n = (tr.meta[nb + node] >> 8) & 0xff;
+                double m = tr.upper[nb + fc];
+                int ties = 1;
+                for (int i = 1; i < n; ++i) {
+                    const double u = tr.upper[nb + fc + i];
+                    if (u > m) { m = u; ties = 1; } else if (u == m) ++ties;
+                }
+                int pick = ties > 1 ? (int)rng.integers((uint32_t)ties) : 0;
+                int child = fc;
+                for (int i = 0; i < n; ++i)
+                    if (tr.upper[nb + fc + i] == m && pick-- == 0) { child = fc + i; break; }
+                action = tr.meta[nb + child] & 0xff;
+            } else {                                 // leaf: "uniform" randint(n_actions) / "zeros" 0
+                action = a.cfg.continuation == 1 ? (int)rng.integers((uint32_t)a.cfg.n_actions) : 0;
+            }
+            // get_child (:155-160): expand a leaf, fall back to the first available action
+            if (fc < 0) {
+                fc = n_nodes;
+                expand_decision(node, amask, h);
+            }
+            const int n = (tr.meta[nb + node] >> 8) & 0xff;
+            int chance = fc;
+            for (int i = 0; i < n; ++i)
+                if ((tr.meta[nb + fc + i] & 0xff) == action) { chance = fc + i; break; }
+            action = tr.meta[nb + chance] & 0xff;
+            bool term;
+            const double r = env.step(a, action, li, gmask, gs, term);          // :82
+            // ChanceNode.get_child (:272-286): placeholders on the first visit, the observation takes placeholder 0
+            int child = tr.first_child[nb + chance];
+            if (child < 0) {
+                child = n_nodes;
+                if (writer) {
+                    for (int i = 0; i < K; ++i) new_node(tr, nb, n_nodes + i, chance, i, KIND_DECISION,
+                                                          a.cfg.init_upper[h + 1]);
+                    tr.first_child[nb + chance] = n_nodes;
+                    tr.meta[nb + chance] = (tr.meta[nb + chance] & ~0xff00) | (K << 8);
+                }
+                n_nodes += K;
+            }
+            if (!(r >= 0.0 && r <= 1.0)) { error = 1; break; }                 // olop.py:133-134
+            if (writer) {
+                tr.count[nb + chance] += 1;                                      // ChanceNode.update (:264-265)
+                int meta = tr.meta[nb + child];                                  // OLOPNode.update (olop.py:132-142)
+                if (term) meta |= DONE_BIT;
+                const double rr = (meta & DONE_BIT) ? 0.0 : r;
+                const double cum = tr.cumulative[nb + child] + rr;
+                const int cnt = tr.count[nb + child] + 1;
+                tr.meta[nb + child] = meta;
+                tr.cumulative[nb + child] = cum;
+                tr.count[nb + child] = cnt;
+                const double thr = a.cfg.thresholds[cnt];                        // compute_reward_ucb (:200-212)
+                tr.mu_ucb[nb + child] = kl_bound(cum, cnt, thr, false);
+                tr.mu_lcb[nb + child] = kl_bound(cum, cnt, thr, true);
+            }
+            __syncwarp(gmask);
+            node = child;
+        }
+        if (error) break;
+        if (writer) {                                                            // backup_to_root
+            int n = node;
+            while (n >= 0) {
+                const int meta = tr.meta[nb + n];
+                const int fc = tr.first_child[nb + n];
+                const int k = (meta >> 8) & 0xff;
+                if (((meta >> KIND_SHIFT) & 1) == KIND_DECISION) {               // :214-226
+                    double up = 0.0, lo = 0.0;                                   // a leaf (depth H): 0 / 0
+                    if (fc >= 0) {
+                        up = tr.upper[nb + fc];
+                        lo = tr.lower[nb + fc];
+                        for (int i = 1; i < k; ++i) {
+                            const double u = tr.upper[nb + fc + i], l = tr.lower[nb + fc + i];
+                            up = u > up ? u : up;
+                            lo = l > lo ? l : lo;
+                        }
+                    }
+                    tr.upper[nb + n] = up;
+                    tr.lower[nb + n] = lo;
+                } else {                                                         // :288-305
+                    const int cnt = tr.count[nb + n];
+                    const double qp = (double)tr.count[nb + fc] / (double)cnt;
+                    const double c = a.cfg.transition_thresholds[cnt] / (double)cnt;
+                    tr.upper[nb + n] = gape_expectation(tr, nb, fc, k, true, gamma, qp, c);
+                    tr.lower[nb + n] = gape_expectation(tr, nb, fc, k, false, gamma, qp, c);
+                }
+                n = tr.parent[nb + n];
+            }
+        }
+        __syncwarp(gmask);
+        int sel;
+        bai(tr, nb, tr.first_child[nb], (tr.meta[nb] >> 8) & 0xff, sel, best, challenger);
+        done = tr.upper[nb + challenger] - tr.lower[nb + best] < a.cfg.accuracy;      // stopping rule (:100-102)
+        done = done || episode > a.cfg.episodes;
+        ++episode;
+    }
+
+    if (writer) {
+        rng.store(a.rng + (int64_t)tree * B2_PCG64_STATE_WORDS);
+        // get_plan (:129-131): the root's BAI best, unchanged since the last episode's selection
+        const int action = error ? -1 : tr.meta[nb + best] & 0xff;
+        a.plan[tree] = (int8_t)action;
+        int32_t* res = a.result + (int64_t)tree * B2_MDP_GAPE_RESULT_WORDS;
+        res[0] = n_nodes;
+        res[1] = episode;
+        res[2] = error;
+        res[3] = action;
+        res[4] = error ? -1 : best;
+        res[5] = error ? -1 : challenger;
+        res[6] = 0;
+        res[7] = 0;
+    }
+}
+
+}  // namespace
+}  // namespace b2
+
+using namespace b2;
+
+extern "C" int b2_mdp_gape_plan(const b2_mdp_gape_config* cfg, const int32_t* root_states, const b2_mdp_gape_tree* tree,
+                                uint64_t* rng, int8_t* plan, int32_t* result, void* stream_) {
+    B2_REQUIRE(cfg && root_states && tree && rng && plan && result, "null pointer");
+    B2_REQUIRE(cfg->n_trees > 0 && cfg->episodes >= 0 && cfg->horizon >= 1, "bad batch / budget");
+    B2_REQUIRE(cfg->n_actions > 0 && cfg->n_actions <= 8, "n_actions must be in 1..8");
+    B2_REQUIRE(cfg->max_next_states >= 1 && cfg->max_next_states <= 255, "max_next_states must be in 1..255");
+    B2_REQUIRE((int64_t)cfg->node_capacity >= 1 + ((int64_t)cfg->episodes + 2) * cfg->horizon *
+                                                      (cfg->n_actions + cfg->max_next_states),
+               "node_capacity too small");
+    B2_REQUIRE(cfg->thresholds && cfg->transition_thresholds && cfg->init_upper,
+               "threshold / initial bound tables missing");
+    cudaStream_t stream = (cudaStream_t)stream_;
+    GapeArgs a;
+    a.cfg = *cfg; a.tree = *tree; a.root_states = root_states; a.rng = rng; a.plan = plan; a.result = result;
+    if (cfg->env_kind == B2_ENV_FINITE) {
+        B2_REQUIRE(cfg->mdp.transition && cfg->mdp.reward && cfg->mdp.terminal, "finite MDP tables missing");
+        B2_REQUIRE(cfg->mdp.n_actions == cfg->n_actions, "mdp.n_actions != n_actions");
+        mdp_gape_kernel<GFiniteEnv><<<(cfg->n_trees + 127) / 128, 128, 0, stream>>>(a);
+    } else if (cfg->env_kind == B2_ENV_HIGHWAY) {
+        B2_REQUIRE(cfg->n_actions == B2_HW_ACTIONS, "HighwayLite has 5 actions");
+        mdp_gape_kernel<GHighwayEnv><<<(cfg->n_trees * 16 + 127) / 128, 128, 0, stream>>>(a);
+    } else {
+        set_error("unknown env_kind %d", cfg->env_kind);
+        return B2_ERR_INVALID;
+    }
+    B2_CUDA_CHECK(cudaGetLastError());
+    return B2_OK;
+}

@@ -15,8 +15,8 @@ def _np_random(seed):
 
 
 def run_batched_episodes(planner, seeds, budget, gamma, max_steps=40, device="cuda", planner_seed=0, **kw):
-    """planner: "opd" | "mcts" | "olop" | "vi" (ValueIterationAgent on the scenes' TTC-grid MDPs, `budget` = its
-    `iterations`).  Every episode: scene make_scene(seed), replanning at every
+    """planner: "opd" | "mcts" | "olop" | "mdp_gape" (keywords: MDPGapEAgent config keys) | "vi" (ValueIterationAgent
+    on the scenes' TTC-grid MDPs, `budget` = its `iterations`).  Every episode: scene make_scene(seed), replanning at every
     step (receding_horizon 1, step_strategy reset -- the reference defaults), until crash or `max_steps`.
     Returns dict(returns, lengths, crashed, decision_ms)."""
     import torch
@@ -42,6 +42,15 @@ def run_batched_episodes(planner, seeds, budget, gamma, max_steps=40, device="cu
         ub = kw.get("upper_bound", {"type": "kullback-leibler", "time": "global", "threshold": "2*np.log(time)"})
         eng = OLOPEngine(_lib.ENV_HIGHWAY, n, 5, episodes, horizon, gamma, ub, kw.get("continuation_type", "uniform"),
                          device=dev)
+    elif planner == "mdp_gape":
+        # MDPGapEAgent's completed config (mdp_gape.py:20-40) with budget / gamma and any keyword overriding it
+        from rl_agents_b200.agents.tree_search.mdp_gape import MDPGapE, budget_allocation
+        from rl_agents_b200.engine.mdp_gape import MDPGapEEngine
+        cfg = MDPGapE.default_config()
+        MDPGapE.rec_update(cfg, dict(kw, budget=budget, gamma=gamma))
+        episodes, horizon = budget_allocation(cfg, 5)
+        eng = MDPGapEEngine(_lib.ENV_HIGHWAY, n, 5, episodes, horizon, gamma, cfg["upper_bound"], cfg["accuracy"],
+                            cfg["confidence"], cfg["continuation_type"], cfg["max_next_states_count"], device=dev)
     elif planner == "vi":
         from rl_agents_b200.engine.ttc_vi import HighwayTTCVI
         eng = HighwayTTCVI(gamma, budget, device=dev)
