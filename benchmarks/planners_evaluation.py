@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Budget sweep of the device planners on HighwayLite (closed loop, batched episodes); one CSV row
 per (planner, budget): mean return, crash rate, mean episode length, ms per batched decision.
-Planners: opd, mcts, olop, vi (ValueIterationAgent on the scenes' TTC-grid MDPs; its "budget" is the
+Planners: opd, mcts, olop, mdp_gape, brue, vi (ValueIterationAgent on the scenes' TTC-grid MDPs; its "budget" is the
 agent's `iterations`, e.g. `--planners vi --budgets 10 --gamma 1.0` = the reference's shipped highway config)."""
 import argparse
 import os

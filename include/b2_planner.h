@@ -533,6 +533,44 @@ typedef struct b2_mdp_gape_tree {
 int b2_mdp_gape_plan(const b2_mdp_gape_config* cfg, const int32_t* root_states, const b2_mdp_gape_tree* tree,
                      uint64_t* rng, int8_t* plan, int32_t* result, void* stream);
 
+/* ------------------------------------------------------------------------
+ * BRUE -- rl_agents/agents/tree_search/brue.py (deterministic env models, so every chance node has exactly one
+ * next-state child).  Incremental means, host gamma**d and arg-maxes only: the trees equal the reference's bit for bit.
+ * ---------------------------------------------------------------------- */
+typedef struct b2_brue_config {
+    int32_t env_kind;
+    int32_t n_trees;
+    int32_t n_actions;       /* action_space.n: rollout actions are randint(n_actions), available or not (:27) */
+    int32_t budget;          /* config["budget"] >= 1: env steps; the last rollout runs to its end (:66-71) */
+    int32_t horizon;         /* config["horizon"] >= 1                         */
+    int32_t node_capacity;   /* per tree, >= 1 + 2 * (budget + horizon - 1)    */
+    double gamma;
+    const double* gamma_pow; /* [horizon] gamma**d (host Python floats, :63)   */
+    b2_finite_mdp mdp;
+} b2_brue_config;
+
+/* One arena for decision and chance nodes; node id = creation order.  A decision node's chance children form a list
+ * first_child -> next_sibling -> ... in creation order (the reference's dict order); a chance node's first_child is
+ * its one decision child. */
+typedef struct b2_brue_tree {
+    int32_t* parent;
+    int32_t* first_child;
+    int32_t* next_sibling;   /* -1 at the end of a list                       */
+    int32_t* count;
+    int32_t* meta;           /* action | kind << 8; action 0xff on decision nodes; kind 0 decision, 1 chance */
+    double* value;           /* ChanceNode.value / DecisionNode.reward (:82-86, :104-108) */
+    int32_t* path;           /* [n_trees, horizon] scratch: the chance nodes of the current rollout */
+    double* path_reward;     /* [n_trees, horizon] scratch: their rewards      */
+} b2_brue_tree;
+
+#define B2_BRUE_RESULT_WORDS 8
+/* per tree int32 result: [0] n_nodes [1] rollouts run [2] env steps taken (budget - available_budget)
+ * [3] recommended action [4] error (1: node_capacity exhausted -- cannot happen at the documented capacity) */
+
+/* BRUE.plan (:66-75); rng as in b2_mcts_plan; plan: int8 [n_trees], the recommended action (-1 on error). */
+int b2_brue_plan(const b2_brue_config* cfg, const int32_t* root_states, const b2_brue_tree* tree, uint64_t* rng,
+                 int8_t* plan, int32_t* result, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

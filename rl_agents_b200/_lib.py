@@ -20,6 +20,7 @@ OPD_RESULT_WORDS = 16
 MCTS_RESULT_WORDS = 8
 OLOP_RESULT_WORDS = 8
 MDP_GAPE_RESULT_WORDS = 8
+BRUE_RESULT_WORDS = 8
 PCG64_STATE_WORDS = 6
 
 
@@ -136,6 +137,19 @@ class MDPGapETree(ctypes.Structure):
     _fields_ = [(n, c_void_p) for n in MDP_GAPE_TREE_FIELDS]
 
 
+class BRUEConfig(ctypes.Structure):
+    _fields_ = [("env_kind", c_int32), ("n_trees", c_int32), ("n_actions", c_int32), ("budget", c_int32),
+                ("horizon", c_int32), ("node_capacity", c_int32), ("gamma", c_double), ("gamma_pow", c_void_p),
+                ("mdp", FiniteMDP)]
+
+
+BRUE_TREE_FIELDS = ("parent", "first_child", "next_sibling", "count", "meta", "value")
+
+
+class BRUETree(ctypes.Structure):
+    _fields_ = [(n, c_void_p) for n in BRUE_TREE_FIELDS + ("path", "path_reward")]
+
+
 EXPORTS = {
     "b2_last_error": (ctypes.c_char_p, []),
     "b2_version": (c_int, []),
@@ -183,6 +197,8 @@ EXPORTS = {
                              c_void_p, c_void_p]),
     "b2_mdp_gape_plan": (c_int, [ctypes.POINTER(MDPGapEConfig), c_void_p, ctypes.POINTER(MDPGapETree), c_void_p,
                                  c_void_p, c_void_p, c_void_p]),
+    "b2_brue_plan": (c_int, [ctypes.POINTER(BRUEConfig), c_void_p, ctypes.POINTER(BRUETree), c_void_p, c_void_p,
+                             c_void_p, c_void_p]),
 }
 
 _lib = None

@@ -15,9 +15,10 @@ def _np_random(seed):
 
 
 def run_batched_episodes(planner, seeds, budget, gamma, max_steps=40, device="cuda", planner_seed=0, **kw):
-    """planner: "opd" | "mcts" | "olop" | "mdp_gape" (keywords: MDPGapEAgent config keys) | "vi" (ValueIterationAgent
-    on the scenes' TTC-grid MDPs, `budget` = its `iterations`).  Every episode: scene make_scene(seed), replanning at every
-    step (receding_horizon 1, step_strategy reset -- the reference defaults), until crash or `max_steps`.
+    """planner: "opd" | "mcts" | "olop" | "mdp_gape" (keywords: MDPGapEAgent config keys) | "brue" (keywords: BRUEAgent
+    config keys) | "vi" (ValueIterationAgent on the scenes' TTC-grid MDPs, `budget` = its `iterations`).  Every
+    episode: scene make_scene(seed), replanning at every step (receding_horizon 1, step_strategy reset -- the reference
+    defaults), until crash or `max_steps`.
     Returns dict(returns, lengths, crashed, decision_ms)."""
     import torch
     from rl_agents_b200.engine.mcts import MCTSEngine, pcg64_words, set_pcg64_words
@@ -51,6 +52,14 @@ def run_batched_episodes(planner, seeds, budget, gamma, max_steps=40, device="cu
         episodes, horizon = budget_allocation(cfg, 5)
         eng = MDPGapEEngine(_lib.ENV_HIGHWAY, n, 5, episodes, horizon, gamma, cfg["upper_bound"], cfg["accuracy"],
                             cfg["confidence"], cfg["continuation_type"], cfg["max_next_states_count"], device=dev)
+    elif planner == "brue":
+        # BRUEAgent's completed config (OLOP's defaults, brue.py:19-22) with budget / gamma and any keyword overriding it
+        from rl_agents_b200.agents.tree_search.brue import BRUE
+        from rl_agents_b200.engine.brue import BRUEEngine
+        cfg = BRUE.default_config()
+        BRUE.rec_update(cfg, dict(kw, budget=budget, gamma=gamma))
+        horizon = cfg["horizon"] if "horizon" in cfg else allocation(max(5, budget), gamma)[1]
+        eng = BRUEEngine(_lib.ENV_HIGHWAY, n, 5, budget, horizon, gamma, device=dev)
     elif planner == "vi":
         from rl_agents_b200.engine.ttc_vi import HighwayTTCVI
         eng = HighwayTTCVI(gamma, budget, device=dev)
