@@ -35,7 +35,7 @@ int b2_device_info(int* sm_count, int* cc_major, int* cc_minor, char* name, int 
 /* ------------------------------------------------------------------------
  * Environment models (the batched transition the planners call)
  * ---------------------------------------------------------------------- */
-#define B2_ENV_FINITE 0   /* deterministic finite MDP tables               */
+#define B2_ENV_FINITE 0   /* finite MDP tables (deterministic, except for sparse sampling) */
 #define B2_ENV_HIGHWAY 1  /* HighwayLite, docs/HIGHWAY_LITE_SPEC.md         */
 
 #define B2_ENV_INTERSECTION 2 /* IntersectionLite, docs/INTERSECTION_LITE_SPEC.md (wavefront OPD + b2_intersection_step) */
@@ -570,6 +570,68 @@ typedef struct b2_brue_tree {
 /* BRUE.plan (:66-75); rng as in b2_mcts_plan; plan: int8 [n_trees], the recommended action (-1 on error). */
 int b2_brue_plan(const b2_brue_config* cfg, const int32_t* root_states, const b2_brue_tree* tree, uint64_t* rng,
                  int8_t* plan, int32_t* result, void* stream);
+
+/* ------------------------------------------------------------------------
+ * Sparse sampling -- rl_agents/agents/tree_search/sparse_sampling.py.  Finite MDPs in all three modes (the sampled
+ * env's `seed(np_random.randint(2**30))` and `Generator.choice(p.size, p=p)` replayed on the device) and HighwayLite.
+ * The values are the reference's fp64 operations in its order: every node equals the reference's bit for bit.
+ * ---------------------------------------------------------------------- */
+/* A finite MDP as the sampled env steps it (FiniteMDPEnv.step): r = reward[s, a]; k = searchsorted(cdf[s, a], u,
+ * "right") for u = default_rng(seed).random(); s' = next[s, a, k]. */
+typedef struct b2_finite_mdp_sampled {
+    int32_t n_states;
+    int32_t n_actions;
+    int32_t n_next;          /* B: 1 "deterministic", S "stochastic" (next[s, a, k] = k), next's width "sparse" */
+    int32_t reserved;
+    const double* cdf;       /* [S, A, B] p.cumsum(); cdf /= cdf[-1], as Generator.choice computes it (host numpy) */
+    const int32_t* next;     /* [S, A, B]                                                                       */
+    const double* reward;    /* [S, A]                                                                          */
+    const uint8_t* row_ok;   /* [S, A] 1 when Generator.choice accepts p[s, a] (no NaN, none negative, Kahan sum
+                                within sqrt(eps) of 1); sampling a row with 0 is the reference's ValueError       */
+} b2_finite_mdp_sampled;
+
+typedef struct b2_sparse_sampling_config {
+    int32_t env_kind;        /* B2_ENV_FINITE or B2_ENV_HIGHWAY                                                 */
+    int32_t n_trees;
+    int32_t n_actions;       /* finite: action_space.n, every action is expanded (the AttributeError fallback of
+                                estimateV, :40-43); HighwayLite: 5, its available actions in env order          */
+    int32_t horizon;         /* config["horizon"] >= 1 (0 leaves the root childless, :45-46)                    */
+    int32_t C;               /* config["C"] >= 1: samples per chance node (:76)                                 */
+    int32_t reserved;
+    double gamma;            /* config["gamma"]: value = reward + gamma * S / C (:87-88)                        */
+    b2_finite_mdp_sampled mdp;   /* env_kind == FINITE                                                          */
+} b2_sparse_sampling_config;
+
+/* Optional creation-order dump of every tree ([n_trees, capacity] each); pass NULL to plan without it. */
+typedef struct b2_sparse_sampling_tree {
+    int32_t capacity;        /* nodes per tree; running out sets error 1                                        */
+    int32_t reserved;
+    int32_t* parent;         /* -1 for the root                                                                 */
+    int32_t* kind;           /* 0 DecisionNode, 1 ChanceNode                                                    */
+    int32_t* key;            /* chance: the action; decision: the next state (finite), -1 (HighwayLite, root)   */
+    int32_t* depth;          /* Node.depth: a chance node has its parent's depth (:34, :68)                     */
+    int32_t* count;          /* DecisionNode.count: samples that reached it (:83); 0 on chance nodes            */
+    double* value;           /* DecisionNode / ChanceNode.value (:51, :87-88)                                   */
+} b2_sparse_sampling_tree;
+
+#define B2_SPARSE_SAMPLING_RESULT_WORDS 8
+/* per tree int32 result: [0] nodes created [1] chance nodes [2] samples drawn (C per chance node) [3] recommended
+ * action (-1 on error) [4] error (1: tree capacity exhausted; 2: a sampled probability row that Generator.choice
+ * rejects) [5] that row, s * n_actions + a (-1 otherwise) */
+
+/* Bytes of scratch the call needs: the depth-first search's stack of `horizon` frames per tree (and, on HighwayLite,
+ * the horizon + 1 env states along the current path). */
+int64_t b2_sparse_sampling_workspace_bytes(const b2_sparse_sampling_config* cfg);
+
+/* SparseSampling.plan (:21-28) for n_trees independent decisions, one tree per lane (finite) or per 16-lane group
+ * (HighwayLite).  Strict depth-first order: per chance node C draws of randint(2**30), the distinct next states in
+ * first-visit order, then their estimateV; the root's tie-break draws choice(indices) (abstract.py:304-311).
+ * rng: uint64 [n_trees, 6] numpy PCG64 states, advanced in place; root_states: [n_trees] state ids or [n_trees, 136]
+ * words; root_q: double [n_trees, n_actions], the root's chance values (NaN for unavailable actions); plan: int8
+ * [n_trees]; tree: NULL or the dump. */
+int b2_sparse_sampling_plan(const b2_sparse_sampling_config* cfg, const int32_t* root_states,
+                            const b2_sparse_sampling_tree* tree, void* workspace, uint64_t* rng, double* root_q,
+                            int8_t* plan, int32_t* result, void* stream);
 
 #ifdef __cplusplus
 }

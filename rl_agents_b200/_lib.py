@@ -21,6 +21,7 @@ MCTS_RESULT_WORDS = 8
 OLOP_RESULT_WORDS = 8
 MDP_GAPE_RESULT_WORDS = 8
 BRUE_RESULT_WORDS = 8
+SPARSE_SAMPLING_RESULT_WORDS = 8
 PCG64_STATE_WORDS = 6
 
 
@@ -150,6 +151,23 @@ class BRUETree(ctypes.Structure):
     _fields_ = [(n, c_void_p) for n in BRUE_TREE_FIELDS + ("path", "path_reward")]
 
 
+class FiniteMDPSampled(ctypes.Structure):
+    _fields_ = [("n_states", c_int32), ("n_actions", c_int32), ("n_next", c_int32), ("reserved", c_int32),
+                ("cdf", c_void_p), ("next", c_void_p), ("reward", c_void_p), ("row_ok", c_void_p)]
+
+
+class SparseSamplingConfig(ctypes.Structure):
+    _fields_ = [("env_kind", c_int32), ("n_trees", c_int32), ("n_actions", c_int32), ("horizon", c_int32),
+                ("C", c_int32), ("reserved", c_int32), ("gamma", c_double), ("mdp", FiniteMDPSampled)]
+
+
+SPARSE_SAMPLING_TREE_FIELDS = ("parent", "kind", "key", "depth", "count", "value")
+
+
+class SparseSamplingTree(ctypes.Structure):
+    _fields_ = [("capacity", c_int32), ("reserved", c_int32)] + [(n, c_void_p) for n in SPARSE_SAMPLING_TREE_FIELDS]
+
+
 EXPORTS = {
     "b2_last_error": (ctypes.c_char_p, []),
     "b2_version": (c_int, []),
@@ -199,6 +217,9 @@ EXPORTS = {
                                  c_void_p, c_void_p, c_void_p]),
     "b2_brue_plan": (c_int, [ctypes.POINTER(BRUEConfig), c_void_p, ctypes.POINTER(BRUETree), c_void_p, c_void_p,
                              c_void_p, c_void_p]),
+    "b2_sparse_sampling_workspace_bytes": (c_int64, [ctypes.POINTER(SparseSamplingConfig)]),
+    "b2_sparse_sampling_plan": (c_int, [ctypes.POINTER(SparseSamplingConfig), c_void_p,
+                                        ctypes.POINTER(SparseSamplingTree)] + [c_void_p] * 6),
 }
 
 _lib = None

@@ -61,6 +61,50 @@ struct Pcg64 {
         }
         return (uint32_t)(m >> 32);
     }
+    // np.random.default_rng(seed) for a seed below 2^32 (an env's `seed(np_random.randint(2**30))`): the words of
+    // SeedSequence(seed).generate_state(4, uint64) -- one entropy word, pool size 4 -- then pcg64_set_seed
+    // (state 0, inc = initseq << 1 | 1, step, state += initstate, step).  CPU twin: oracle/seed_sequence.py.
+    __device__ __forceinline__ void seed_from(uint32_t seed) {
+        uint32_t hash_const = 0x43B0D7E5u;
+        auto hashmix = [&hash_const](uint32_t v) {
+            v ^= hash_const;
+            hash_const *= 0x931E8875u;
+            v *= hash_const;
+            return v ^ (v >> 16);
+        };
+        auto mix = [](uint32_t x, uint32_t y) {
+            const uint32_t r = 0xCA01F9DDu * x - 0x4973F715u * y;
+            return r ^ (r >> 16);
+        };
+        uint32_t pool[4];
+        pool[0] = hashmix(seed);
+#pragma unroll
+        for (int i = 1; i < 4; ++i) pool[i] = hashmix(0u);
+#pragma unroll
+        for (int src = 0; src < 4; ++src)
+#pragma unroll
+            for (int dst = 0; dst < 4; ++dst)
+                if (src != dst) pool[dst] = mix(pool[dst], hashmix(pool[src]));
+        uint32_t hb = 0x8B51F9DDu, w[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+            uint32_t v = pool[i & 3] ^ hb;
+            hb *= 0x58F38DEDu;
+            v *= hb;
+            w[i] = v ^ (v >> 16);
+        }
+        const unsigned __int128 initstate = ((unsigned __int128)(((uint64_t)w[1] << 32) | w[0]) << 64) |
+                                            (((uint64_t)w[3] << 32) | w[2]);
+        const unsigned __int128 initseq = ((unsigned __int128)(((uint64_t)w[5] << 32) | w[4]) << 64) |
+                                          (((uint64_t)w[7] << 32) | w[6]);
+        state = 0;
+        inc = (initseq << 1) | 1u;
+        next64();
+        state += initstate;
+        next64();
+        has_uint32 = 0;
+        uinteger = 0;
+    }
 };
 
 }  // namespace b2

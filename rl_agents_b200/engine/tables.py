@@ -52,6 +52,72 @@ def preference_tables(n_actions, ratio):
     return prior, cdf
 
 
+def choice_rows_ok(p):
+    """Per row of p [..., B]: whether Generator.choice(B, p=row) accepts it -- its Kahan sum is not NaN, no entry is
+    negative, and the sum is within sqrt(eps) of 1."""
+    p = np.asarray(p, dtype=np.float64)
+    total, comp = p[..., 0].copy(), np.zeros(p.shape[:-1])
+    with np.errstate(invalid="ignore", over="ignore"):
+        for i in range(1, p.shape[-1]):          # numpy's kahan_sum, row by row
+            y = p[..., i] - comp
+            t = total + y
+            comp = (t - total) - y
+            total = t
+        bad = np.isnan(total) | (p < 0).any(axis=-1) | (np.abs(total - 1.0) > np.sqrt(np.finfo(np.float64).eps))
+    return ~bad
+
+
+def sampled_mdp_tables(mdp):
+    """A finite MDP as its env steps it (FiniteMDPEnv.step): r = reward[s, a]; k = Generator.choice(B, p=p[s, a]) of
+    the env's freshly seeded generator, i.e. searchsorted(cdf, random(), "right") with the cdf numpy builds
+    (p.cumsum(); cdf /= cdf[-1]); s' = next[s, a, k].  "deterministic": B = 1, next = transition; "stochastic":
+    B = S, next[s, a, k] = k; "sparse": the given next.  -> dict(cdf, next, reward, row_ok)."""
+    reward = np.ascontiguousarray(mdp.reward, dtype=np.float64)
+    S, A = reward.shape
+    if mdp.mode == "deterministic":
+        nxt = np.asarray(mdp.transition).reshape(S, A, 1)
+        cdf = np.ones((S, A, 1))
+        ok = np.ones((S, A), dtype=bool)
+    elif mdp.mode in ("stochastic", "sparse"):
+        p = np.asarray(mdp.transition, dtype=np.float64)
+        if mdp.mode == "stochastic":
+            nxt = np.broadcast_to(np.arange(p.shape[-1]), p.shape)
+        else:
+            nxt = np.asarray(mdp.next)
+        with np.errstate(invalid="ignore", divide="ignore"):
+            cdf = p.cumsum(axis=-1)
+            cdf /= cdf[..., -1:]
+        ok = choice_rows_ok(p)
+    else:
+        raise ValueError("Unknown mode %r" % (mdp.mode,))
+    if nxt.shape != cdf.shape or (nxt.size and (nxt.min() < 0 or nxt.max() >= S)):
+        raise ValueError("next states must be an [S, A, B] table of state ids")
+    return {"cdf": np.ascontiguousarray(cdf), "next": np.ascontiguousarray(nxt, dtype=np.int32), "reward": reward,
+            "row_ok": np.ascontiguousarray(ok, dtype=np.uint8)}
+
+
+class SampledFiniteTables(object):
+    """Device copy of a finite MDP in any mode, for the planners that sample transitions (sparse sampling)."""
+
+    def __init__(self, mdp, device):
+        import torch
+        self.mode = mdp.mode
+        t = sampled_mdp_tables(mdp)
+        self.p = None if mdp.mode == "deterministic" else np.asarray(mdp.transition, dtype=np.float64)
+        self.n_states, self.n_actions, self.n_next = t["cdf"].shape
+        for k, v in t.items():
+            setattr(self, k, torch.as_tensor(v, device=device))
+
+    def row(self, row):
+        """The probability row s * A + a, as Generator.choice reads it."""
+        return self.p.reshape(-1, self.p.shape[-1])[row]
+
+    def struct(self):
+        from rl_agents_b200 import _lib
+        return _lib.FiniteMDPSampled(self.n_states, self.n_actions, self.n_next, 0, self.cdf.data_ptr(),
+                                     self.next.data_ptr(), self.reward.data_ptr(), self.row_ok.data_ptr())
+
+
 class FiniteTables(object):
     """Device copy of a deterministic finite MDP (int32 transitions)."""
 

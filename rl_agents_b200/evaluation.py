@@ -16,7 +16,8 @@ def _np_random(seed):
 
 def run_batched_episodes(planner, seeds, budget, gamma, max_steps=40, device="cuda", planner_seed=0, **kw):
     """planner: "opd" | "mcts" | "olop" | "mdp_gape" (keywords: MDPGapEAgent config keys) | "brue" (keywords: BRUEAgent
-    config keys) | "vi" (ValueIterationAgent on the scenes' TTC-grid MDPs, `budget` = its `iterations`).  Every
+    config keys) | "sparse_sampling" (keywords `horizon` and `C`, required as in SparseSamplingAgent's config; `budget`
+    is unused) | "vi" (ValueIterationAgent on the scenes' TTC-grid MDPs, `budget` = its `iterations`).  Every
     episode: scene make_scene(seed), replanning at every step (receding_horizon 1, step_strategy reset -- the reference
     defaults), until crash or `max_steps`.
     Returns dict(returns, lengths, crashed, decision_ms)."""
@@ -60,6 +61,9 @@ def run_batched_episodes(planner, seeds, budget, gamma, max_steps=40, device="cu
         BRUE.rec_update(cfg, dict(kw, budget=budget, gamma=gamma))
         horizon = cfg["horizon"] if "horizon" in cfg else allocation(max(5, budget), gamma)[1]
         eng = BRUEEngine(_lib.ENV_HIGHWAY, n, 5, budget, horizon, gamma, device=dev)
+    elif planner == "sparse_sampling":
+        from rl_agents_b200.engine.sparse_sampling import SparseSamplingEngine
+        eng = SparseSamplingEngine(_lib.ENV_HIGHWAY, n, 5, kw["horizon"], kw["C"], gamma, device=dev)
     elif planner == "vi":
         from rl_agents_b200.engine.ttc_vi import HighwayTTCVI
         eng = HighwayTTCVI(gamma, budget, device=dev)
