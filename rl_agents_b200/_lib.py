@@ -110,8 +110,11 @@ class MCTSWaveTree(ctypes.Structure):
     _fields_ = [(n, c_void_p) for n in ("parent", "first_child", "count", "meta", "vsum", "value")]
 
 
+MCTS_TREE_FIELDS = ("parent", "first_child", "count", "meta", "value", "prior")
+
+
 class MCTSTree(ctypes.Structure):
-    _fields_ = [(n, c_void_p) for n in ("parent", "first_child", "count", "meta", "value", "prior")]
+    _fields_ = [(n, c_void_p) for n in MCTS_TREE_FIELDS]
 
 
 class OLOPConfig(ctypes.Structure):
@@ -120,8 +123,11 @@ class OLOPConfig(ctypes.Structure):
                 ("gamma", c_double), ("thresholds", c_void_p), ("init_upper", c_void_p), ("mdp", FiniteMDP)]
 
 
+OLOP_TREE_FIELDS = ("parent", "first_child", "count", "meta", "cumulative", "mu_ucb", "upper")
+
+
 class OLOPTree(ctypes.Structure):
-    _fields_ = [(n, c_void_p) for n in ("parent", "first_child", "count", "meta", "cumulative", "mu_ucb", "upper")]
+    _fields_ = [(n, c_void_p) for n in OLOP_TREE_FIELDS]
 
 
 class MDPGapEConfig(ctypes.Structure):

@@ -35,12 +35,11 @@ class DiscreteRobustPlanner(AbstractPlanner):
         width = max(1, int(self.config.get("wavefront", 1) or 1))          # 1: the reference's strict order
         key = (d0.kind, d0.n_actions, len(models), self.config["budget"], self.config["gamma"],
                self.config.get("terminal_reward", 0), width, tuple(mdp_fingerprint(d.mdp) for d in descs))
-        if key != self._engine_key:
-            self.engine = OPDWaveEngine(d0.kind, d0.n_actions, self.config["budget"], self.config["gamma"], width,
-                                        self.config.get("terminal_reward", 0), n_models=len(models),
-                                        model_mdps=[d.mdp for d in descs] if d0.mdp is not None else None)
-            self._engine_key = key
-        eng = self.engine
+        eng = self.cached_engine(key, lambda: OPDWaveEngine(d0.kind, d0.n_actions, self.config["budget"],
+                                                            self.config["gamma"], width,
+                                                            self.config.get("terminal_reward", 0), n_models=len(models),
+                                                            model_mdps=[d.mdp for d in descs] if d0.mdp is not None
+                                                            else None))
         root = torch.from_numpy(np.ascontiguousarray(np.stack([d.root.reshape(-1) for d in descs]))).to(eng.device)
         eng.plan(root.contiguous())
         plans, _ = eng.finish([self.np_random])

@@ -25,6 +25,13 @@ def np_random(seed=None):
     return np.random.Generator(np.random.PCG64(seed_seq)), seed_seq.entropy
 
 
+def refuse_intersection(name, env):
+    """BRUE, MDP-GapE and sparse sampling model finite MDPs and HighwayLite only: refuse an IntersectionLite env, both
+    when the planner is built and when it is handed the env to plan on."""
+    if getattr(getattr(env, "unwrapped", env), "b2_env_kind", None) == "intersection":
+        raise NotImplementedError("%s runs on finite MDPs and HighwayLite, not on IntersectionLite" % name)
+
+
 class _OpenLoopQueue(object):
     """Receding-horizon bookkeeping of a tree-search agent.
 
@@ -139,6 +146,25 @@ class AbstractPlanner(Configurable):
 
     def plan(self, state, observation):
         raise NotImplementedError()
+
+    def cached_engine(self, key, make):
+        """The engine make() built for `key`; a new one only when the key differs from the last call's."""
+        if key != self._engine_key:
+            self.engine = make()
+            self._engine_key = key
+        return self.engine
+
+    def search_one_tree(self, engine, d, *plan_args):
+        """One tree from the root of `d` (describe()) on the planner's own PCG64 stream, which the device
+        advances -> (plan, result words of the tree)."""
+        import torch
+        from rl_agents_b200.engine.mcts import pcg64_words, set_pcg64_words
+        root = torch.from_numpy(d.root.reshape(1, -1) if d.root.size > 1 else d.root).to(engine.device)
+        engine.plan(root.contiguous(), pcg64_words(self.np_random).reshape(1, -1), *plan_args)
+        plans, res, rng_words = engine.finish()
+        set_pcg64_words(self.np_random, rng_words[0])
+        self.last_tree = engine
+        return plans[0], res[0]
 
     def get_visits(self):
         return defaultdict(int)

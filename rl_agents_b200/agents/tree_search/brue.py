@@ -1,8 +1,7 @@
 """BRUE agent on the device engine.  Drop-in for rl_agents.agents.tree_search.brue.BRUEAgent (brue.py:11-123) with
 step_strategy "reset"."""
-from rl_agents_b200 import _lib
 from rl_agents_b200.agents.common.abstract import register_with_reference
-from rl_agents_b200.agents.tree_search.abstract import AbstractTreeSearchAgent
+from rl_agents_b200.agents.tree_search.abstract import AbstractTreeSearchAgent, refuse_intersection
 from rl_agents_b200.agents.tree_search.olop import OLOP
 from rl_agents_b200.envs.adapters import describe, mdp_fingerprint
 
@@ -20,37 +19,24 @@ class BRUE(OLOP):
         # the reference's "subtree" re-roots on a chance node, whose next plan() raises AttributeError
         if self.config["step_strategy"] == "subtree":
             raise NotImplementedError("BRUE on the device supports step_strategy 'reset' only")
-        if getattr(getattr(env, "unwrapped", env), "b2_env_kind", None) == "intersection":
-            raise NotImplementedError("BRUE runs on finite MDPs and HighwayLite, not on IntersectionLite")
-
-    def _engine_for(self, d):
-        from rl_agents_b200.engine.brue import BRUEEngine
-        c = self.config
-        key = (d.kind, d.n_actions, c["budget"], c["horizon"], c["gamma"], mdp_fingerprint(d.mdp))
-        if key != self._engine_key:
-            self.engine = BRUEEngine(d.kind, 1, d.n_actions, c["budget"], c["horizon"], c["gamma"], mdp=d.mdp)
-            self._engine_key = key
-        return self.engine
+        refuse_intersection("BRUE", env)
 
     def plan(self, state, observation):
-        import torch
-        from rl_agents_b200.engine.mcts import pcg64_words, set_pcg64_words
+        from rl_agents_b200.engine.brue import BRUEEngine
         if self.config["horizon"] < 1:
             # the reference's rollouts would never take a step, so its budget loop would never end
             raise ValueError("BRUE needs horizon >= 1 (got %r)" % self.config["horizon"])
         if self.config["budget"] < 1:
             raise ValueError(EMPTY_ROOT_MESSAGE)                     # no rollout: get_plan has nothing to choose
         d = describe(state)
-        if d.kind == _lib.ENV_INTERSECTION:
-            raise NotImplementedError("BRUE runs on finite MDPs and HighwayLite, not on IntersectionLite")
-        eng = self._engine_for(d)
-        root = torch.from_numpy(d.root.reshape(1, -1) if d.root.size > 1 else d.root).to(eng.device)
-        eng.plan(root.contiguous(), pcg64_words(self.np_random).reshape(1, -1))
-        plans, res, rng_words = eng.finish()
-        set_pcg64_words(self.np_random, rng_words[0])
-        self.available_budget = self.config["budget"] - int(res[0, 2])     # <= 0: the last rollout overshoots
-        self.last_tree = eng
-        return plans[0]
+        refuse_intersection("BRUE", state)
+        c = self.config
+        key = (d.kind, d.n_actions, c["budget"], c["horizon"], c["gamma"], mdp_fingerprint(d.mdp))
+        eng = self.cached_engine(key, lambda: BRUEEngine(d.kind, 1, d.n_actions, c["budget"], c["horizon"], c["gamma"],
+                                                         mdp=d.mdp))
+        plan, res = self.search_one_tree(eng, d)
+        self.available_budget = self.config["budget"] - int(res[2])        # <= 0: the last rollout overshoots
+        return plan
 
 
 @register_with_reference

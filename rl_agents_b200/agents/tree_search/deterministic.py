@@ -48,19 +48,18 @@ class OptimisticDeterministicPlanner(AbstractPlanner):
             width = max(width, 1)          # IntersectionLite lives in the whole-GPU kernels (width 1 = strict order)
         key = (d.kind, d.n_actions, self.config["budget"], self.config["gamma"],
                self.config.get("terminal_reward", 0), width, spec, mdp_fingerprint(d.mdp))
-        if key != self._engine_key:
+
+        def make():
             if spec > 0:
-                self.engine = OPDSpeculativeEngine(d.kind, d.n_actions, self.config["budget"], self.config["gamma"],
-                                                   spec, self.config.get("terminal_reward", 0), mdp=d.mdp)
-            elif width > 0:
-                self.engine = OPDWaveEngine(d.kind, d.n_actions, self.config["budget"], self.config["gamma"], width,
+                return OPDSpeculativeEngine(d.kind, d.n_actions, self.config["budget"], self.config["gamma"], spec,
                                             self.config.get("terminal_reward", 0), mdp=d.mdp)
-            else:
-                self.engine = OPDEngine(d.kind, 1, d.n_actions, self.config["budget"], self.config["gamma"],
-                                        self.config.get("terminal_reward", 0), mdp=d.mdp,
-                                        keys_in_smem=self.config.get("keys_in_smem", True))
-            self._engine_key = key
-        return self.engine
+            if width > 0:
+                return OPDWaveEngine(d.kind, d.n_actions, self.config["budget"], self.config["gamma"], width,
+                                     self.config.get("terminal_reward", 0), mdp=d.mdp)
+            return OPDEngine(d.kind, 1, d.n_actions, self.config["budget"], self.config["gamma"],
+                             self.config.get("terminal_reward", 0), mdp=d.mdp,
+                             keys_in_smem=self.config.get("keys_in_smem", True))
+        return self.cached_engine(key, make)
 
     def plan(self, state, observation):
         import torch

@@ -12,24 +12,16 @@ class GraphBasedPlanner(AbstractPlanner):
         self.env = env
 
     def plan(self, state, observation):
-        import torch
         from rl_agents_b200.engine.gbop import GBOPDEngine
-        from rl_agents_b200.engine.mcts import pcg64_words, set_pcg64_words
         d = describe(state)
         if d.kind != _lib.ENV_FINITE:
             raise TypeError("the device GBOP-D planner builds a graph over state ids: it needs a finite-MDP env")
         key = (d.n_actions, self.config["budget"], self.config["gamma"], self.config["accuracy"],
                self.config["sampling_timeout"], mdp_fingerprint(d.mdp))
-        if key != self._engine_key:
-            self.engine = GBOPDEngine(1, d.n_actions, self.config["budget"], self.config["gamma"], d.mdp,
-                                      self.config["accuracy"], self.config["sampling_timeout"])
-            self._engine_key = key
-        eng = self.engine
-        eng.plan(torch.from_numpy(d.root).to(eng.device).contiguous(), pcg64_words(self.np_random).reshape(1, -1))
-        plans, _, words = eng.finish()
-        set_pcg64_words(self.np_random, words[0])          # the tie-breaks consumed the planner's stream
-        self.last_tree = eng
-        return plans[0]
+        eng = self.cached_engine(key, lambda: GBOPDEngine(1, d.n_actions, self.config["budget"], self.config["gamma"],
+                                                          d.mdp, self.config["accuracy"],
+                                                          self.config["sampling_timeout"]))
+        return self.search_one_tree(eng, d)[0]          # the tie-breaks consume the planner's stream
 
 
 @register_with_reference

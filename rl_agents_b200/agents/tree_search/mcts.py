@@ -48,18 +48,19 @@ class MCTS(AbstractPlanner):
         from rl_agents_b200.engine.mcts import MCTSEngine
         key = (d.kind, d.n_actions, replicas, episodes, self.config["horizon"], self.config["gamma"],
                self.config["temperature"], repr(self.rollout_policy), repr(self.prior_policy), mdp_fingerprint(d.mdp))
-        if key != self._engine_key:
+
+        def make():
             # "subtree" keeps nodes alive for up to `horizon` decisions (a node at depth d survives d re-rootings)
             capacity = None
             if self.config["step_strategy"] == "subtree":
                 capacity = 1 + (self.config["horizon"] + 1) * episodes * d.n_actions
-            self.engine = MCTSEngine(d.kind, replicas, d.n_actions, episodes, self.config["horizon"],
-                                     self.config["gamma"], self.config["temperature"], mdp=d.mdp,
-                                     rollout_policy=self.rollout_policy, prior_policy=self.prior_policy,
-                                     capacity=capacity)
-            self._engine_key = key
+            engine = MCTSEngine(d.kind, replicas, d.n_actions, episodes, self.config["horizon"],
+                                self.config["gamma"], self.config["temperature"], mdp=d.mdp,
+                                rollout_policy=self.rollout_policy, prior_policy=self.prior_policy,
+                                capacity=capacity)
             self._resume = 0
-        return self.engine
+            return engine
+        return self.cached_engine(key, make)
 
     def reset(self):
         super(MCTS, self).reset()
@@ -81,7 +82,7 @@ class MCTS(AbstractPlanner):
 
     def plan(self, state, observation):
         import torch
-        from rl_agents_b200.engine.mcts import pcg64_words, set_pcg64_words
+        from rl_agents_b200.engine.mcts import pcg64_words
         d = describe(state)
         replicas = int(self.config.get("root_parallel", 1) or 1)
         root = torch.from_numpy(d.root.reshape(1, -1) if d.root.size > 1 else d.root)
@@ -95,11 +96,9 @@ class MCTS(AbstractPlanner):
                 raise NotImplementedError("wavefront MCTS implements the random_available policies")
             key = ("wave", d.kind, d.n_actions, self.config["episodes"], self.config["horizon"], self.config["gamma"],
                    self.config["temperature"], width, mdp_fingerprint(d.mdp))
-            if key != self._engine_key:
-                self.engine = MCTSWaveEngine(d.kind, d.n_actions, self.config["episodes"], self.config["horizon"],
-                                             self.config["gamma"], self.config["temperature"], width, mdp=d.mdp)
-                self._engine_key = key
-            eng = self.engine
+            eng = self.cached_engine(key, lambda: MCTSWaveEngine(d.kind, d.n_actions, self.config["episodes"],
+                                                                 self.config["horizon"], self.config["gamma"],
+                                                                 self.config["temperature"], width, mdp=d.mdp))
             seed = int(self.np_random.integers(0, 2 ** 63 - 1))
             eng.plan(root.reshape(-1).to(eng.device).contiguous(), seed)
             plan, _ = eng.finish()
@@ -111,12 +110,9 @@ class MCTS(AbstractPlanner):
             # the reference's semantics: one tree, strict episode order, the planner's own RNG stream
             eng = self._engine_for(d, 1, self.config["episodes"])
             resume = [self._resume] if getattr(self, "_resume", 0) > 0 else None
-            eng.plan(root.to(eng.device).contiguous(), pcg64_words(self.np_random).reshape(1, -1), resume)
+            plan, _ = self.search_one_tree(eng, d, resume)
             self._resume = 0
-            plans, res, rng_words = eng.finish()
-            set_pcg64_words(self.np_random, rng_words[0])     # the device consumed the planner's stream
-            self.last_tree = eng
-            return plans[0]
+            return plan
         # extension ("root_parallel": R): R independent trees of episodes/R episodes from the same root,
         # each on its own spawned stream; root statistics merged as in rl_agents_b200.distributed
         from rl_agents_b200.distributed import recommend

@@ -2,10 +2,9 @@
 rl_agents.agents.tree_search.mdp_gape.MDPGapEAgent (mdp_gape.py:11-344) with step_strategy "reset"."""
 import numpy as np
 
-from rl_agents_b200 import _lib
 from rl_agents_b200.agents.common.abstract import register_with_reference
 from rl_agents_b200.agents.common.factory import preprocess_env
-from rl_agents_b200.agents.tree_search.abstract import AbstractPlanner, AbstractTreeSearchAgent
+from rl_agents_b200.agents.tree_search.abstract import AbstractPlanner, AbstractTreeSearchAgent, refuse_intersection
 from rl_agents_b200.agents.tree_search.mcts import allocation
 from rl_agents_b200.envs.adapters import describe, mdp_fingerprint
 
@@ -34,8 +33,7 @@ class MDPGapE(AbstractPlanner):
             raise NotImplementedError("MDP-GapE on the device supports step_strategy 'reset' only")
         if self.config["upper_bound"]["type"] != "kullback-leibler":
             raise NotImplementedError("MDP-GapE supports the kullback-leibler upper bound only")
-        if getattr(getattr(env, "unwrapped", env), "b2_env_kind", None) == "intersection":
-            raise NotImplementedError("MDP-GapE runs on finite MDPs and HighwayLite, not on IntersectionLite")
+        refuse_intersection("MDP-GapE", env)
 
     @classmethod
     def default_config(cls):
@@ -59,34 +57,22 @@ class MDPGapE(AbstractPlanner):
             self.config["episodes"], self.config["horizon"] = budget_allocation(self.config, self.env.action_space.n)
         super(MDPGapE, self).reset()
 
-    def _engine_for(self, d):
+    def plan(self, state, observation):
         from rl_agents_b200.engine.mdp_gape import MDPGapEEngine
+        d = describe(state)
+        refuse_intersection("MDP-GapE", state)
         c = self.config
         ub = c["upper_bound"]
         key = (d.kind, d.n_actions, c["episodes"], c["horizon"], c["gamma"], c["accuracy"], c["confidence"],
                c["continuation_type"], c["max_next_states_count"], ub["type"], ub["threshold"],
                ub["transition_threshold"], mdp_fingerprint(d.mdp))
-        if key != self._engine_key:
-            self.engine = MDPGapEEngine(d.kind, 1, d.n_actions, c["episodes"], c["horizon"], c["gamma"], ub,
-                                        c["accuracy"], c["confidence"], c["continuation_type"],
-                                        c["max_next_states_count"], mdp=d.mdp)
-            self._engine_key = key
-        return self.engine
-
-    def plan(self, state, observation):
-        import torch
-        from rl_agents_b200.engine.mcts import pcg64_words, set_pcg64_words
-        d = describe(state)
-        if d.kind == _lib.ENV_INTERSECTION:
-            raise NotImplementedError("MDP-GapE runs on finite MDPs and HighwayLite, not on IntersectionLite")
-        eng = self._engine_for(d)
-        root = torch.from_numpy(d.root.reshape(1, -1) if d.root.size > 1 else d.root).to(eng.device)
-        eng.plan(root.contiguous(), pcg64_words(self.np_random).reshape(1, -1))
-        plans, res, rng_words = eng.finish()
-        set_pcg64_words(self.np_random, rng_words[0])
-        self.budget_used = int(res[0, 1]) * self.config["horizon"]          # mdp_gape.py:109
-        self.last_tree = eng
-        return plans[0]
+        eng = self.cached_engine(key, lambda: MDPGapEEngine(d.kind, 1, d.n_actions, c["episodes"], c["horizon"],
+                                                            c["gamma"], ub, c["accuracy"], c["confidence"],
+                                                            c["continuation_type"], c["max_next_states_count"],
+                                                            mdp=d.mdp))
+        plan, res = self.search_one_tree(eng, d)
+        self.budget_used = int(res[1]) * self.config["horizon"]             # mdp_gape.py:109
+        return plan
 
 
 @register_with_reference

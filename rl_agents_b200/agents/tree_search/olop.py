@@ -24,28 +24,16 @@ class OLOP(AbstractPlanner):
             self.config["episodes"], self.config["horizon"] = allocation(budget, self.config["gamma"])
         super(OLOP, self).reset()
 
-    def _engine_for(self, d):
+    def plan(self, state, observation):
         from rl_agents_b200.engine.olop import OLOPEngine
+        d = describe(state)
         ub = self.config["upper_bound"]
         key = (d.kind, d.n_actions, self.config["episodes"], self.config["horizon"], self.config["gamma"],
                ub["type"], ub["time"], ub["threshold"], self.config["continuation_type"], mdp_fingerprint(d.mdp))
-        if key != self._engine_key:
-            self.engine = OLOPEngine(d.kind, 1, d.n_actions, self.config["episodes"], self.config["horizon"],
-                                     self.config["gamma"], ub, self.config["continuation_type"], mdp=d.mdp)
-            self._engine_key = key
-        return self.engine
-
-    def plan(self, state, observation):
-        import torch
-        from rl_agents_b200.engine.mcts import pcg64_words, set_pcg64_words
-        d = describe(state)
-        eng = self._engine_for(d)
-        root = torch.from_numpy(d.root.reshape(1, -1) if d.root.size > 1 else d.root).to(eng.device)
-        eng.plan(root.contiguous(), pcg64_words(self.np_random).reshape(1, -1))
-        plans, res, rng_words = eng.finish()
-        set_pcg64_words(self.np_random, rng_words[0])
-        self.last_tree = eng
-        return plans[0]
+        eng = self.cached_engine(key, lambda: OLOPEngine(d.kind, 1, d.n_actions, self.config["episodes"],
+                                                         self.config["horizon"], self.config["gamma"], ub,
+                                                         self.config["continuation_type"], mdp=d.mdp))
+        return self.search_one_tree(eng, d)[0]
 
 
 @register_with_reference

@@ -1,9 +1,8 @@
 """Sparse-sampling agent on the device engine.  Drop-in for
 rl_agents.agents.tree_search.sparse_sampling.SparseSamplingAgent (sparse_sampling.py:11-103) with step_strategy
 "reset", on finite MDPs in every mode ("deterministic", "stochastic", "sparse") and on HighwayLite."""
-from rl_agents_b200 import _lib
 from rl_agents_b200.agents.common.abstract import register_with_reference
-from rl_agents_b200.agents.tree_search.abstract import AbstractPlanner, AbstractTreeSearchAgent
+from rl_agents_b200.agents.tree_search.abstract import AbstractPlanner, AbstractTreeSearchAgent, refuse_intersection
 from rl_agents_b200.envs.adapters import describe, mdp_fingerprint
 
 
@@ -17,38 +16,24 @@ class SparseSampling(AbstractPlanner):
         # the reference's "subtree" re-roots on a chance node, whose next plan() fails
         if self.config["step_strategy"] == "subtree":
             raise NotImplementedError("sparse sampling on the device supports step_strategy 'reset' only")
-        if getattr(getattr(env, "unwrapped", env), "b2_env_kind", None) == "intersection":
-            raise NotImplementedError("sparse sampling runs on finite MDPs and HighwayLite, not on IntersectionLite")
+        refuse_intersection("sparse sampling", env)
         self.root_values = None
 
-    def _engine_for(self, d, horizon, C):
-        from rl_agents_b200.engine.sparse_sampling import SparseSamplingEngine
-        key = (d.kind, d.n_actions, horizon, C, self.config["gamma"], mdp_fingerprint(d.mdp))
-        if key != self._engine_key:
-            self.engine = SparseSamplingEngine(d.kind, 1, d.n_actions, horizon, C, self.config["gamma"], mdp=d.mdp)
-            self._engine_key = key
-        return self.engine
-
     def plan(self, state, observation):
-        import torch
-        from rl_agents_b200.engine.mcts import pcg64_words, set_pcg64_words
-        from rl_agents_b200.engine.sparse_sampling import EMPTY_ROOT_MESSAGE, check_horizon_and_c
+        from rl_agents_b200.engine.sparse_sampling import EMPTY_ROOT_MESSAGE, SparseSamplingEngine, check_horizon_and_c
         horizon = self.config["horizon"]            # KeyError without one, as the reference's estimateV (:45)
         if horizon == 0:
             raise ValueError(EMPTY_ROOT_MESSAGE)    # a childless root, before C is ever read
         C = self.config["C"]                        # KeyError without one, as estimateQ (:76)
         check_horizon_and_c(horizon, C)
         d = describe(state)
-        if d.kind == _lib.ENV_INTERSECTION:
-            raise NotImplementedError("sparse sampling runs on finite MDPs and HighwayLite, not on IntersectionLite")
-        eng = self._engine_for(d, horizon, C)
-        root = torch.from_numpy(d.root.reshape(1, -1) if d.root.size > 1 else d.root).to(eng.device)
-        eng.plan(root.contiguous(), pcg64_words(self.np_random).reshape(1, -1))
-        plans, res, rng_words = eng.finish()
-        set_pcg64_words(self.np_random, rng_words[0])
+        refuse_intersection("sparse sampling", state)
+        key = (d.kind, d.n_actions, horizon, C, self.config["gamma"], mdp_fingerprint(d.mdp))
+        eng = self.cached_engine(key, lambda: SparseSamplingEngine(d.kind, 1, d.n_actions, horizon, C,
+                                                                   self.config["gamma"], mdp=d.mdp))
+        plan, _ = self.search_one_tree(eng, d)
         self.root_values = eng.root_q[0].cpu().numpy()       # the root's chance values by action (NaN: unavailable)
-        self.last_tree = eng
-        return plans[0]
+        return plan
 
 
 @register_with_reference

@@ -28,12 +28,10 @@ class StateAwarePlanner(AbstractPlanner):
         key = (d.n_actions, self.config["budget"], self.config["gamma"], self.config.get("terminal_reward", 0),
                self.config["backup_aggregated_nodes"], self.config["prune_suboptimal_leaves"], self.config["accuracy"],
                mdp_fingerprint(d.mdp))
-        if key != self._engine_key:
-            self.engine = GBOPEngine(1, d.n_actions, self.config["budget"], self.config["gamma"], d.mdp,
-                                     self.config.get("terminal_reward", 0), self.config["backup_aggregated_nodes"],
-                                     self.config["prune_suboptimal_leaves"], self.config["accuracy"])
-            self._engine_key = key
-        eng = self.engine
+        eng = self.cached_engine(key, lambda: GBOPEngine(1, d.n_actions, self.config["budget"], self.config["gamma"],
+                                                         d.mdp, self.config.get("terminal_reward", 0),
+                                                         self.config["backup_aggregated_nodes"],
+                                                         self.config["prune_suboptimal_leaves"], self.config["accuracy"]))
         eng.plan(torch.from_numpy(d.root).to(eng.device).contiguous())
         plans, _ = eng.finish([self.np_random])
         self.last_tree = eng

@@ -15,7 +15,7 @@
 // whose budget is spent leaves its loop; hw::step only synchronises the 16 lanes of one group, so the other tree
 // of the warp carries on.
 #include "common.cuh"
-#include "highway_lite.cuh"
+#include "lane_env.cuh"
 #include "pcg64.cuh"
 
 namespace b2 {
@@ -67,32 +67,6 @@ __device__ double estimate(const b2_brue_tree& tr, int64_t nb, int node, int lev
     return ret;
 }
 
-struct BFiniteEnv {
-    static constexpr int GROUP = 1;
-    int s;
-    __device__ __forceinline__ void load_root(const BrueArgs& a, int tree, int li) { s = a.root_states[tree]; }
-    __device__ __forceinline__ double step(const BrueArgs& a, int action, int li, unsigned gmask, float* gs, bool& term) {
-        const b2_finite_mdp& m = a.cfg.mdp;
-        const double r = m.reward[(int64_t)s * m.n_actions + action];
-        term = m.terminal[s] != 0;        // done = terminal[state BEFORE the transition]
-        s = m.transition[(int64_t)s * m.n_actions + action];
-        return r;
-    }
-};
-
-struct BHighwayEnv {
-    static constexpr int GROUP = 16;
-    hw::Lane L;
-    int t, si;
-    __device__ __forceinline__ void load_root(const BrueArgs& a, int tree, int li) {
-        hw::load_state(a.root_states + (int64_t)tree * hw::WORDS, li, L, t, si);
-    }
-    __device__ __forceinline__ double step(const BrueArgs& a, int action, int li, unsigned gmask, float* gs, bool& term) {
-        bool trunc;                       // the reference's 4-tuple step drops truncation
-        return (double)hw::step(L, li, t, si, action, term, trunc, gmask, gs);
-    }
-};
-
 template <class Env>
 __global__ void __launch_bounds__(128, 8) brue_kernel(BrueArgs a) {
     constexpr int G = Env::GROUP;
@@ -121,13 +95,13 @@ __global__ void __launch_bounds__(128, 8) brue_kernel(BrueArgs a) {
         if (G > 1) error = __shfl_sync(gmask, error, 0, G);
         if (error) break;
         Env env;
-        env.load_root(a, tree, li);                  // safe_deepcopy_env(state), :69
+        env.load_root(a.root_states, tree, li);      // safe_deepcopy_env(state), :69
         rng.integers(1u << 30);                      // state.seed(np_random.randint(2**30)), :25
         int node = 0, len = 0;
         for (int h = 0; h < H; ++h) {                // rollout (:24-33)
             const int action = (int)rng.integers((uint32_t)a.cfg.n_actions);
-            bool term;
-            const double r = env.step(a, action, li, gmask, gs, term);
+            bool term, trunc;
+            const double r = env.step(a.cfg.mdp, action, li, gmask, gs, term, trunc);
             if (writer) {                            // update's forward pass (:39-44)
                 // DecisionNode.get_child: the chance child of this action, appended to the list on the first visit
                 int c = tr.first_child[nb + node], last = -1;
@@ -215,20 +189,15 @@ extern "C" int b2_brue_plan(const b2_brue_config* cfg, const int32_t* root_state
     B2_REQUIRE((int64_t)cfg->node_capacity >= 1 + 2 * ((int64_t)cfg->budget + cfg->horizon - 1),
                "node_capacity too small");
     B2_REQUIRE(cfg->gamma_pow, "gamma**d table missing");
+    const int rc = check_lane_env(cfg->env_kind, cfg->n_actions, cfg->mdp);
+    if (rc != B2_OK) return rc;
     cudaStream_t stream = (cudaStream_t)stream_;
     BrueArgs a;
     a.cfg = *cfg; a.tree = *tree; a.root_states = root_states; a.rng = rng; a.plan = plan; a.result = result;
-    if (cfg->env_kind == B2_ENV_FINITE) {
-        B2_REQUIRE(cfg->mdp.transition && cfg->mdp.reward && cfg->mdp.terminal, "finite MDP tables missing");
-        B2_REQUIRE(cfg->mdp.n_actions == cfg->n_actions, "mdp.n_actions != n_actions");
-        brue_kernel<BFiniteEnv><<<(cfg->n_trees + 127) / 128, 128, 0, stream>>>(a);
-    } else if (cfg->env_kind == B2_ENV_HIGHWAY) {
-        B2_REQUIRE(cfg->n_actions == B2_HW_ACTIONS, "HighwayLite has 5 actions");
-        brue_kernel<BHighwayEnv><<<(cfg->n_trees * 16 + 127) / 128, 128, 0, stream>>>(a);
-    } else {
-        set_error("unknown env_kind %d", cfg->env_kind);
-        return B2_ERR_INVALID;
-    }
+    if (cfg->env_kind == B2_ENV_FINITE)
+        brue_kernel<FiniteEnv><<<lane_grid(cfg->n_trees, FiniteEnv::GROUP), 128, 0, stream>>>(a);
+    else
+        brue_kernel<HighwayEnv><<<lane_grid(cfg->n_trees, HighwayEnv::GROUP), 128, 0, stream>>>(a);
     B2_CUDA_CHECK(cudaGetLastError());
     return B2_OK;
 }

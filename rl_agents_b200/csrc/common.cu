@@ -17,6 +17,24 @@ int sm_count() {
     if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
     return n;
 }
+
+int check_env_kind(int env_kind, int n_actions) {
+    if (env_kind == B2_ENV_FINITE) return B2_OK;
+    if (env_kind != B2_ENV_HIGHWAY) {
+        set_error("unknown env_kind %d", env_kind);
+        return B2_ERR_INVALID;
+    }
+    B2_REQUIRE(n_actions == B2_HW_ACTIONS, "HighwayLite has 5 actions");
+    return B2_OK;
+}
+
+int check_lane_env(int env_kind, int n_actions, const b2_finite_mdp& mdp) {
+    if (env_kind == B2_ENV_FINITE) {
+        B2_REQUIRE(mdp.transition && mdp.reward && mdp.terminal, "finite MDP tables missing");
+        B2_REQUIRE(mdp.n_actions == n_actions, "mdp.n_actions != n_actions");
+    }
+    return check_env_kind(env_kind, n_actions);
+}
 }  // namespace b2
 
 extern "C" const char* b2_last_error(void) { return b2::g_err; }

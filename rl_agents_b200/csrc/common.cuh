@@ -30,6 +30,15 @@ void set_error(const char* fmt, ...);
 
 int sm_count();
 
+// Launch checks of the planners that run one tree per lane group.  Both return B2_OK, or B2_ERR_INVALID with the
+// error set.  check_env_kind: a known env_kind, and HighwayLite's 5 actions; check_lane_env also requires the
+// finite tables and their action count.
+int check_env_kind(int env_kind, int n_actions);
+int check_lane_env(int env_kind, int n_actions, const b2_finite_mdp& mdp);
+
+// Blocks of 128 threads for n_trees trees of `group` lanes each.
+inline int lane_grid(int n_trees, int group) { return (n_trees * group + 127) / 128; }
+
 __device__ __forceinline__ double warp_max_f64(double v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {

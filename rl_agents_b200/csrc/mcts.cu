@@ -10,7 +10,7 @@
 // mcts.py:183), 1 lane for finite MDPs.  Tree bookkeeping is group-uniform
 // scalar code; lane 0 of the group performs the stores.
 #include "common.cuh"
-#include "highway_lite.cuh"
+#include "lane_env.cuh"
 #include "pcg64.cuh"
 
 namespace b2 {
@@ -24,53 +24,6 @@ struct MctsArgs {
     uint64_t* rng;
     int8_t* plan;
     int32_t* result;
-};
-
-// ---------------------------------------------------------------- envs ----
-struct FiniteEnv {
-    static constexpr int GROUP = 1;
-    int s;
-    __device__ __forceinline__ void load_root(const MctsArgs& a, int tree, int li) { s = a.root_states[tree]; }
-    __device__ __forceinline__ int avail(const MctsArgs& a, unsigned gmask) const { return (1 << a.cfg.n_actions) - 1; }
-    __device__ __forceinline__ static int nth(int mask, int n) { return n; }
-    // position of `action` among the available actions in the env's order, or -1
-    __device__ __forceinline__ static int rank_of(int mask, int action) { return (action >= 0 && (mask >> action) & 1) ? action : -1; }
-    __device__ __forceinline__ double step(const MctsArgs& a, int action, int li, unsigned gmask, float* gs, bool& term, bool& trunc) {
-        const b2_finite_mdp& m = a.cfg.mdp;
-        const double r = m.reward[(int64_t)s * m.n_actions + action];
-        term = m.terminal[s] != 0;        // finite_mdp's MDP.step: done = terminal[state BEFORE the transition]
-        s = m.transition[(int64_t)s * m.n_actions + action];
-        trunc = false;
-        return r;
-    }
-};
-
-struct HighwayEnv {
-    static constexpr int GROUP = 16;
-    hw::Lane L;
-    int t, si;
-    __device__ __forceinline__ void load_root(const MctsArgs& a, int tree, int li) {
-        hw::load_state(a.root_states + (int64_t)tree * hw::WORDS, li, L, t, si);
-    }
-    __device__ __forceinline__ int avail(const MctsArgs& a, unsigned gmask) const {
-        const float ego_y = __shfl_sync(gmask, L.y, 0, 16);
-        return hw::avail_mask(ego_y, si);
-    }
-    __device__ __forceinline__ static int nth(int mask, int n) { return hw::nth_action(mask, n); }
-    __device__ __forceinline__ static int rank_of(int mask, int action) {
-        if (action < 0 || !((mask >> action) & 1)) return -1;
-        const int order[5] = {hw::A_IDLE, hw::A_LEFT, hw::A_RIGHT, hw::A_FASTER, hw::A_SLOWER};
-        int k = 0;
-#pragma unroll
-        for (int i = 0; i < 5; ++i) {
-            if (order[i] == action) return k;
-            k += (mask >> order[i]) & 1;
-        }
-        return -1;
-    }
-    __device__ __forceinline__ double step(const MctsArgs& a, int action, int li, unsigned gmask, float* gs, bool& term, bool& trunc) {
-        return (double)hw::step(L, li, t, si, action, term, trunc, gmask, gs);
-    }
 };
 
 // --------------------------------------------------------------- kernel ---
@@ -104,7 +57,7 @@ __global__ void __launch_bounds__(128, B2_MCTS_MIN_BLOCKS) mcts_kernel(MctsArgs 
 
     for (int ep = 0; ep < a.cfg.episodes; ++ep) {
         Env env;
-        env.load_root(a, tree, li);                 // safe_deepcopy_env(state), mcts.py:183
+        env.load_root(a.root_states, tree, li);     // safe_deepcopy_env(state), mcts.py:183
         int node = 0;
         bool in_sel = true, active = live;
         double total = 0.0;
@@ -113,7 +66,7 @@ __global__ void __launch_bounds__(128, B2_MCTS_MIN_BLOCKS) mcts_kernel(MctsArgs 
             // other half of the warp keeps stepping its own scene under its half mask
             if (!active) break;
             int action = hw::A_IDLE < A ? hw::A_IDLE : 0, child = -1;
-            const int amask = env.avail(a, gmask);
+            const int amask = env.avail(a.cfg.n_actions, gmask);
             if (active && in_sel && tr.first_child[nb + node] < 0) {
                 // expansion (mcts.py:151-154, :237-246): children for the policy's actions
                 const int pm = a.cfg.prior_policy != 1 ? amask : (1 << A) - 1;
@@ -182,7 +135,7 @@ __global__ void __launch_bounds__(128, B2_MCTS_MIN_BLOCKS) mcts_kernel(MctsArgs 
             }
             bool term, trunc;
             Env next = env;
-            const double r = next.step(a, action, li, gmask, scratch[(threadIdx.x >> 4) % (128 / 16)], term, trunc);
+            const double r = next.step(a.cfg.mdp, action, li, gmask, scratch[(threadIdx.x >> 4) % (128 / 16)], term, trunc);
             if (active) {
                 env = next;
                 ++env_steps;
@@ -248,22 +201,15 @@ extern "C" int b2_mcts_plan(const b2_mcts_config* cfg, const int32_t* root_state
                "policy must be 0 (random_available), 1 (random) or 2 (preference)");
     B2_REQUIRE((cfg->prior_policy != 2 || cfg->pref_prior) && (cfg->rollout_policy != 2 || cfg->pref_cdf),
                "preference policy tables missing");
+    const int rc = check_lane_env(cfg->env_kind, cfg->n_actions, cfg->mdp);
+    if (rc != B2_OK) return rc;
     cudaStream_t stream = (cudaStream_t)stream_;
     MctsArgs a;
     a.cfg = *cfg; a.tree = *tree; a.root_states = root_states; a.rng = rng; a.plan = plan; a.result = result;
-    if (cfg->env_kind == B2_ENV_FINITE) {
-        B2_REQUIRE(cfg->mdp.transition && cfg->mdp.reward && cfg->mdp.terminal, "finite MDP tables missing");
-        B2_REQUIRE(cfg->mdp.n_actions == cfg->n_actions, "mdp.n_actions != n_actions");
-        const int grid = (cfg->n_trees + 127) / 128;
-        mcts_kernel<FiniteEnv><<<grid, 128, 0, stream>>>(a);
-    } else if (cfg->env_kind == B2_ENV_HIGHWAY) {
-        B2_REQUIRE(cfg->n_actions == B2_HW_ACTIONS, "HighwayLite has 5 actions");
-        const int grid = (cfg->n_trees * 16 + 127) / 128;
-        mcts_kernel<HighwayEnv><<<grid, 128, 0, stream>>>(a);
-    } else {
-        set_error("unknown env_kind %d", cfg->env_kind);
-        return B2_ERR_INVALID;
-    }
+    if (cfg->env_kind == B2_ENV_FINITE)
+        mcts_kernel<FiniteEnv><<<lane_grid(cfg->n_trees, FiniteEnv::GROUP), 128, 0, stream>>>(a);
+    else
+        mcts_kernel<HighwayEnv><<<lane_grid(cfg->n_trees, HighwayEnv::GROUP), 128, 0, stream>>>(a);
     B2_CUDA_CHECK(cudaGetLastError());
     return B2_OK;
 }

@@ -17,8 +17,8 @@
 // itself from the tree arrays; lane 0 writes the tree.  A tree whose stopping rule fired leaves its episode
 // loop; hw::step only synchronises the 16 lanes of one group, so the other trees of the warp carry on.
 #include "common.cuh"
-#include "highway_lite.cuh"
 #include "kl_bound.cuh"
+#include "lane_env.cuh"
 #include "pcg64.cuh"
 
 namespace b2 {
@@ -119,38 +119,6 @@ __device__ __forceinline__ void new_node(const b2_mdp_gape_tree& tr, int64_t nb,
     tr.upper[nb + id] = init_upper; tr.lower[nb + id] = 0.0;
 }
 
-struct GFiniteEnv {
-    static constexpr int GROUP = 1;
-    int s;
-    __device__ __forceinline__ void load_root(const GapeArgs& a, int tree, int li) { s = a.root_states[tree]; }
-    __device__ __forceinline__ int avail(const GapeArgs& a, unsigned gmask) const { return (1 << a.cfg.n_actions) - 1; }
-    __device__ __forceinline__ static int nth(int mask, int n) { return n; }
-    __device__ __forceinline__ double step(const GapeArgs& a, int action, int li, unsigned gmask, float* gs, bool& term) {
-        const b2_finite_mdp& m = a.cfg.mdp;
-        const double r = m.reward[(int64_t)s * m.n_actions + action];
-        term = m.terminal[s] != 0;        // done = terminal[state BEFORE the transition]
-        s = m.transition[(int64_t)s * m.n_actions + action];
-        return r;
-    }
-};
-
-struct GHighwayEnv {
-    static constexpr int GROUP = 16;
-    hw::Lane L;
-    int t, si;
-    __device__ __forceinline__ void load_root(const GapeArgs& a, int tree, int li) {
-        hw::load_state(a.root_states + (int64_t)tree * hw::WORDS, li, L, t, si);
-    }
-    __device__ __forceinline__ int avail(const GapeArgs& a, unsigned gmask) const {
-        return hw::avail_mask(__shfl_sync(gmask, L.y, 0, 16), si);
-    }
-    __device__ __forceinline__ static int nth(int mask, int n) { return hw::nth_action(mask, n); }
-    __device__ __forceinline__ double step(const GapeArgs& a, int action, int li, unsigned gmask, float* gs, bool& term) {
-        bool trunc;
-        return (double)hw::step(L, li, t, si, action, term, trunc, gmask, gs);
-    }
-};
-
 template <class Env>
 __global__ void __launch_bounds__(128, 8) mdp_gape_kernel(GapeArgs a) {
     constexpr int G = Env::GROUP;
@@ -189,12 +157,12 @@ __global__ void __launch_bounds__(128, 8) mdp_gape_kernel(GapeArgs a) {
 
     while (!done) {                                  // MDPGapE.plan (:94-110)
         Env env;
-        env.load_root(a, tree, li);                  // safe_deepcopy_env(state), :98
+        env.load_root(a.root_states, tree, li);      // safe_deepcopy_env(state), :98
         rng.integers(1u << 30);                      // state.seed(np_random.randint(2**30)), :67
-        if (tr.first_child[nb] < 0) expand_decision(0, env.avail(a, gmask), 0);
+        if (tr.first_child[nb] < 0) expand_decision(0, env.avail(a.cfg.n_actions, gmask), 0);
         int node = 0;
         for (int h = 0; h < H; ++h) {
-            const int amask = env.avail(a, gmask);
+            const int amask = env.avail(a.cfg.n_actions, gmask);
             int fc = tr.first_child[nb + node];
             // sampling_rule (:183-198)
             int action;
@@ -230,8 +198,8 @@ __global__ void __launch_bounds__(128, 8) mdp_gape_kernel(GapeArgs a) {
             for (int i = 0; i < n; ++i)
                 if ((tr.meta[nb + fc + i] & 0xff) == action) { chance = fc + i; break; }
             action = tr.meta[nb + chance] & 0xff;
-            bool term;
-            const double r = env.step(a, action, li, gmask, gs, term);          // :82
+            bool term, trunc;
+            const double r = env.step(a.cfg.mdp, action, li, gmask, gs, term, trunc);          // :82
             // ChanceNode.get_child (:272-286): placeholders on the first visit, the observation takes placeholder 0
             int child = tr.first_child[nb + chance];
             if (child < 0) {
@@ -333,20 +301,15 @@ extern "C" int b2_mdp_gape_plan(const b2_mdp_gape_config* cfg, const int32_t* ro
                "node_capacity too small");
     B2_REQUIRE(cfg->thresholds && cfg->transition_thresholds && cfg->init_upper,
                "threshold / initial bound tables missing");
+    const int rc = check_lane_env(cfg->env_kind, cfg->n_actions, cfg->mdp);
+    if (rc != B2_OK) return rc;
     cudaStream_t stream = (cudaStream_t)stream_;
     GapeArgs a;
     a.cfg = *cfg; a.tree = *tree; a.root_states = root_states; a.rng = rng; a.plan = plan; a.result = result;
-    if (cfg->env_kind == B2_ENV_FINITE) {
-        B2_REQUIRE(cfg->mdp.transition && cfg->mdp.reward && cfg->mdp.terminal, "finite MDP tables missing");
-        B2_REQUIRE(cfg->mdp.n_actions == cfg->n_actions, "mdp.n_actions != n_actions");
-        mdp_gape_kernel<GFiniteEnv><<<(cfg->n_trees + 127) / 128, 128, 0, stream>>>(a);
-    } else if (cfg->env_kind == B2_ENV_HIGHWAY) {
-        B2_REQUIRE(cfg->n_actions == B2_HW_ACTIONS, "HighwayLite has 5 actions");
-        mdp_gape_kernel<GHighwayEnv><<<(cfg->n_trees * 16 + 127) / 128, 128, 0, stream>>>(a);
-    } else {
-        set_error("unknown env_kind %d", cfg->env_kind);
-        return B2_ERR_INVALID;
-    }
+    if (cfg->env_kind == B2_ENV_FINITE)
+        mdp_gape_kernel<FiniteEnv><<<lane_grid(cfg->n_trees, FiniteEnv::GROUP), 128, 0, stream>>>(a);
+    else
+        mdp_gape_kernel<HighwayEnv><<<lane_grid(cfg->n_trees, HighwayEnv::GROUP), 128, 0, stream>>>(a);
     B2_CUDA_CHECK(cudaGetLastError());
     return B2_OK;
 }

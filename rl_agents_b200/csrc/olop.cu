@@ -9,8 +9,8 @@
 // Same lane-group mapping as mcts.cu: one tree per 16-lane group (HighwayLite,
 // lane = vehicle slot) or per lane (finite MDP).
 #include "common.cuh"
-#include "highway_lite.cuh"
 #include "kl_bound.cuh"
+#include "lane_env.cuh"
 #include "pcg64.cuh"
 
 namespace b2 {
@@ -22,38 +22,6 @@ struct OlopArgs {
     uint64_t* rng;
     int8_t* plan;
     int32_t* result;
-};
-
-struct OFiniteEnv {
-    static constexpr int GROUP = 1;
-    int s;
-    __device__ __forceinline__ void load_root(const OlopArgs& a, int tree, int li) { s = a.root_states[tree]; }
-    __device__ __forceinline__ int avail(const OlopArgs& a, unsigned gmask) const { return (1 << a.cfg.n_actions) - 1; }
-    __device__ __forceinline__ static int nth(int mask, int n) { return n; }
-    __device__ __forceinline__ double step(const OlopArgs& a, int action, int li, unsigned gmask, float* gs, bool& term) {
-        const b2_finite_mdp& m = a.cfg.mdp;
-        const double r = m.reward[(int64_t)s * m.n_actions + action];
-        term = m.terminal[s] != 0;        // done = terminal[state BEFORE the transition]
-        s = m.transition[(int64_t)s * m.n_actions + action];
-        return r;
-    }
-};
-
-struct OHighwayEnv {
-    static constexpr int GROUP = 16;
-    hw::Lane L;
-    int t, si;
-    __device__ __forceinline__ void load_root(const OlopArgs& a, int tree, int li) {
-        hw::load_state(a.root_states + (int64_t)tree * hw::WORDS, li, L, t, si);
-    }
-    __device__ __forceinline__ int avail(const OlopArgs& a, unsigned gmask) const {
-        return hw::avail_mask(__shfl_sync(gmask, L.y, 0, 16), si);
-    }
-    __device__ __forceinline__ static int nth(int mask, int n) { return hw::nth_action(mask, n); }
-    __device__ __forceinline__ double step(const OlopArgs& a, int action, int li, unsigned gmask, float* gs, bool& term) {
-        bool trunc;
-        return (double)hw::step(L, li, t, si, action, term, trunc, gmask, gs);
-    }
 };
 
 template <class Env>
@@ -83,13 +51,13 @@ __global__ void __launch_bounds__(128, 8) olop_kernel(OlopArgs a) {
 
     for (int ep = 0; ep < a.cfg.episodes; ++ep) {
         Env env;
-        env.load_root(a, tree, li);                 // safe_deepcopy_env(state), olop.py:98
+        env.load_root(a.root_states, tree, li);     // safe_deepcopy_env(state), olop.py:98
         if (live) rng.integers(1u << 30);            // state.seed(np_random.randint(2**30)), :73
         int node = 0;
         const double threshold = a.cfg.thresholds[ep];
         for (int h = 0; h < L; ++h) {
             int action = 0, child = 0;
-            const int amask = env.avail(a, gmask);
+            const int amask = env.avail(a.cfg.n_actions, gmask);
             if (live && !error) {
                 int fc = tr.first_child[nb + node];
                 if (fc < 0) {
@@ -129,8 +97,9 @@ __global__ void __launch_bounds__(128, 8) olop_kernel(OlopArgs a) {
                 }
                 action = tr.meta[nb + child] & 0xff;
             }
-            bool term;
-            const double r = env.step(a, action, li, gmask, scratch[(threadIdx.x >> 4) % (128 / 16)], term);     // olop.py:87
+            bool term, trunc;
+            const double r = env.step(a.cfg.mdp, action, li, gmask, scratch[(threadIdx.x >> 4) % (128 / 16)], term,
+                                      trunc);     // olop.py:87
             if (live && !error) {
                 node = child;
                 // update (olop.py:132-142)
@@ -207,20 +176,15 @@ extern "C" int b2_olop_plan(const b2_olop_config* cfg, const int32_t* root_state
     B2_REQUIRE((int64_t)cfg->node_capacity >= 1 + (int64_t)cfg->episodes * cfg->horizon * cfg->n_actions,
                "node_capacity too small");
     B2_REQUIRE(cfg->thresholds && cfg->init_upper, "threshold / initial bound tables missing");
+    const int rc = check_lane_env(cfg->env_kind, cfg->n_actions, cfg->mdp);
+    if (rc != B2_OK) return rc;
     cudaStream_t stream = (cudaStream_t)stream_;
     OlopArgs a;
     a.cfg = *cfg; a.tree = *tree; a.root_states = root_states; a.rng = rng; a.plan = plan; a.result = result;
-    if (cfg->env_kind == B2_ENV_FINITE) {
-        B2_REQUIRE(cfg->mdp.transition && cfg->mdp.reward && cfg->mdp.terminal, "finite MDP tables missing");
-        B2_REQUIRE(cfg->mdp.n_actions == cfg->n_actions, "mdp.n_actions != n_actions");
-        olop_kernel<OFiniteEnv><<<(cfg->n_trees + 127) / 128, 128, 0, stream>>>(a);
-    } else if (cfg->env_kind == B2_ENV_HIGHWAY) {
-        B2_REQUIRE(cfg->n_actions == B2_HW_ACTIONS, "HighwayLite has 5 actions");
-        olop_kernel<OHighwayEnv><<<(cfg->n_trees * 16 + 127) / 128, 128, 0, stream>>>(a);
-    } else {
-        set_error("unknown env_kind %d", cfg->env_kind);
-        return B2_ERR_INVALID;
-    }
+    if (cfg->env_kind == B2_ENV_FINITE)
+        olop_kernel<FiniteEnv><<<lane_grid(cfg->n_trees, FiniteEnv::GROUP), 128, 0, stream>>>(a);
+    else
+        olop_kernel<HighwayEnv><<<lane_grid(cfg->n_trees, HighwayEnv::GROUP), 128, 0, stream>>>(a);
     B2_CUDA_CHECK(cudaGetLastError());
     return B2_OK;
 }

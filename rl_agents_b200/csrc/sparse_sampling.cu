@@ -338,20 +338,18 @@ extern "C" int b2_sparse_sampling_plan(const b2_sparse_sampling_config* cfg, con
         a.tree = *tree;
     }
     a.root_states = root_states; a.rng = rng; a.root_q = root_q; a.plan = plan; a.result = result;
+    const int rc = check_env_kind(cfg->env_kind, cfg->n_actions);
+    if (rc != B2_OK) return rc;
     cudaStream_t stream = (cudaStream_t)stream_;
     if (cfg->env_kind == B2_ENV_FINITE) {
         const b2_finite_mdp_sampled& m = cfg->mdp;
         B2_REQUIRE(m.cdf && m.next && m.reward && m.row_ok, "finite MDP tables missing");
         B2_REQUIRE(m.n_actions == cfg->n_actions && m.n_states > 0 && m.n_next >= 1, "bad finite MDP shape");
         layout((char*)workspace, cfg->n_trees, cfg->horizon, cfg->C, false, a.st);
-        sparse_sampling_kernel<SFiniteEnv><<<(cfg->n_trees + 127) / 128, 128, 0, stream>>>(a);
-    } else if (cfg->env_kind == B2_ENV_HIGHWAY) {
-        B2_REQUIRE(cfg->n_actions == B2_HW_ACTIONS, "HighwayLite has 5 actions");
-        layout((char*)workspace, cfg->n_trees, cfg->horizon, cfg->C, true, a.st);
-        sparse_sampling_kernel<SHighwayEnv><<<(cfg->n_trees * 16 + 127) / 128, 128, 0, stream>>>(a);
+        sparse_sampling_kernel<SFiniteEnv><<<lane_grid(cfg->n_trees, SFiniteEnv::GROUP), 128, 0, stream>>>(a);
     } else {
-        set_error("unknown env_kind %d", cfg->env_kind);
-        return B2_ERR_INVALID;
+        layout((char*)workspace, cfg->n_trees, cfg->horizon, cfg->C, true, a.st);
+        sparse_sampling_kernel<SHighwayEnv><<<lane_grid(cfg->n_trees, SHighwayEnv::GROUP), 128, 0, stream>>>(a);
     }
     B2_CUDA_CHECK(cudaGetLastError());
     return B2_OK;

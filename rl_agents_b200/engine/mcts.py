@@ -3,6 +3,7 @@ import numpy as np
 
 from rl_agents_b200 import _lib
 from rl_agents_b200.engine.tables import FiniteTables, gamma_tables, preference_tables, uniform_cdf_table
+from rl_agents_b200.engine.tree_engine import TreeEngine, decode_action
 
 POLICIES = {"random_available": 0, "random": 1, "preference": 2}
 
@@ -70,33 +71,24 @@ def reroot_arrays(arrays, n, action):
     return out, len(order)
 
 
-class MCTSEngine(object):
+class MCTSEngine(TreeEngine):
     """n_trees independent MCTS decisions per launch; every tree consumes its
     own numpy PCG64 stream exactly as the reference planner would."""
 
     def __init__(self, env_kind, n_trees, n_actions, episodes, horizon, gamma, temperature, mdp=None,
                  rollout_policy="random_available", prior_policy="random_available", device="cuda", capacity=None):
-        import torch
-        self.torch = torch
-        self.lib = _lib.load()
-        self.device = torch.device(device)
+        super(MCTSEngine, self).__init__(n_trees, _lib.MCTS_RESULT_WORDS, device)
+        torch = self.torch
         rollout_id, rollout_action, rollout_ratio = policy_spec(rollout_policy)
         prior_id, prior_action, prior_ratio = policy_spec(prior_policy)
-        self.n_trees, self.n_actions = int(n_trees), int(n_actions)
+        self.n_actions = int(n_actions)
         self.episodes, self.horizon = int(episodes), int(horizon)
         self.capacity = max(int(capacity or 0), 1 + self.episodes * self.n_actions)
         gp, _ = gamma_tables(gamma, self.horizon + 1)
         self.gamma_pow = torch.as_tensor(gp, device=self.device)
         self.cdf = torch.as_tensor(uniform_cdf_table(self.n_actions), device=self.device)
         self.tables = FiniteTables(mdp, self.device) if env_kind == _lib.ENV_FINITE else None
-        shape = (self.n_trees, self.capacity)
-        i32, f64 = torch.int32, torch.float64
-        self.parent = torch.empty(shape, dtype=i32, device=self.device)
-        self.first_child = torch.empty(shape, dtype=i32, device=self.device)
-        self.count = torch.empty(shape, dtype=i32, device=self.device)
-        self.meta = torch.empty(shape, dtype=i32, device=self.device)
-        self.value = torch.empty(shape, dtype=f64, device=self.device)
-        self.prior = torch.empty(shape, dtype=f64, device=self.device)
+        self.tree = _lib.MCTSTree(*self._alloc_tree(_lib.MCTS_TREE_FIELDS, self.capacity))
         self.pref_prior = torch.as_tensor(preference_tables(self.n_actions, prior_ratio)[0], device=self.device)
         self.pref_cdf = torch.as_tensor(preference_tables(self.n_actions, rollout_ratio)[1], device=self.device)
         self.cfg = _lib.MCTSConfig(env_kind, self.n_trees, self.n_actions, self.episodes, self.horizon, self.capacity,
@@ -104,17 +96,13 @@ class MCTSEngine(object):
                                    self.gamma_pow.data_ptr(), self.cdf.data_ptr(),
                                    self.tables.struct() if self.tables else _lib.FiniteMDP(),
                                    prior_action, rollout_action, self.pref_prior.data_ptr(), self.pref_cdf.data_ptr(), None)
-        self.resume = torch.zeros(self.n_trees, dtype=i32, device=self.device)
-        self.tree = _lib.MCTSTree(*[t.data_ptr() for t in (self.parent, self.first_child, self.count, self.meta,
-                                                           self.value, self.prior)])
+        self.resume = torch.zeros(self.n_trees, dtype=torch.int32, device=self.device)
         self.plan_buf = torch.empty((self.n_trees, max(self.horizon, 1)), dtype=torch.int8, device=self.device)
-        self.result = torch.empty((self.n_trees, _lib.MCTS_RESULT_WORDS), dtype=i32, device=self.device)
-        self.rng = torch.empty((self.n_trees, _lib.PCG64_STATE_WORDS), dtype=torch.int64, device=self.device)
 
     def plan(self, root_states, rng_words, resume_nodes=None):
         """rng_words: uint64 [n_trees, 6] numpy (pcg64_words per tree).  resume_nodes: per-tree node counts of
         re-rooted sub-trees already in the arrays (see reroot), or None for fresh trees."""
-        self.rng.copy_(self.torch.from_numpy(np.ascontiguousarray(rng_words).view(np.int64)))
+        self._load_rng(rng_words)
         if resume_nodes is None:
             self.cfg.resume_nodes = None
         else:
@@ -123,18 +111,15 @@ class MCTSEngine(object):
         _lib.check(self.lib.b2_mcts_plan(self.cfg, _lib.ptr(root_states), self.tree, _lib.ptr(self.rng),
                                          _lib.ptr(self.plan_buf), _lib.ptr(self.result), _lib.current_stream()))
 
-    def finish(self):
-        """Synchronise; returns (plans, result array, advanced rng words)."""
-        res = self.result.cpu().numpy()
-        plans_dev = self.plan_buf.cpu().numpy()
-        plans = [plans_dev[i, :res[i, 1]].astype(int).tolist() for i in range(self.n_trees)]
-        return plans, res, self.rng.cpu().numpy().view(np.uint64)
+    def _plans(self, res):
+        plans = self.plan_buf.cpu().numpy()
+        return [plans[i, :res[i, 1]].astype(int).tolist() for i in range(self.n_trees)]
 
     def reroot(self, tree, action):
         """Keep the sub-tree under root child `action` of `tree` (host-side compaction, once per decision).
         Returns the number of nodes kept (0: the action was never expanded -> start a new tree)."""
         n = int(self.result[tree, 0].item())
-        names = ("parent", "first_child", "count", "meta", "value", "prior")
+        names = _lib.MCTS_TREE_FIELDS
         arrays = {k: getattr(self, k)[tree, :n].cpu().numpy() for k in names}
         out, kept = reroot_arrays(arrays, n, int(action))
         if kept + self.episodes * self.n_actions > self.capacity:
@@ -146,9 +131,7 @@ class MCTSEngine(object):
     def tree_dict(self, tree=0):
         n = int(self.result[tree, 0].item())
         meta = self.meta[tree, :n].cpu().numpy()
-        action = (meta & 0xff).astype(int)
-        action[action == 0xff] = -1
-        return {"parent": self.parent[tree, :n].cpu().numpy(), "action": action,
+        return {"parent": self.parent[tree, :n].cpu().numpy(), "action": decode_action(meta),
                 "count": self.count[tree, :n].cpu().numpy(), "value": self.value[tree, :n].cpu().numpy(),
                 "prior": self.prior[tree, :n].cpu().numpy(),
                 "first_child": self.first_child[tree, :n].cpu().numpy(), "n_children": (meta >> 8) & 0xff}
@@ -202,9 +185,7 @@ class MCTSWaveEngine(object):
 
     def tree_dict(self):
         meta = self.meta.cpu().numpy()
-        action = (meta & 0xff).astype(int)
-        action[action == 0xff] = -1
-        return {"parent": self.parent.cpu().numpy(), "action": action, "count": self.count.cpu().numpy(),
+        return {"parent": self.parent.cpu().numpy(), "action": decode_action(meta), "count": self.count.cpu().numpy(),
                 "first_child": self.first_child.cpu().numpy(), "n_children": (meta >> 8) & 0xff,
                 "vsum": self.vsum.cpu().numpy(), "value": self.value.cpu().numpy()}
 

@@ -3,6 +3,7 @@ import numpy as np
 
 from rl_agents_b200 import _lib
 from rl_agents_b200.engine.tables import FiniteTables
+from rl_agents_b200.engine.tree_engine import TreeEngine, decode_action
 
 
 def count_table(expression, episodes, horizon, n_actions, confidence):
@@ -16,20 +17,18 @@ def count_table(expression, episodes, horizon, n_actions, confidence):
     return out
 
 
-class MDPGapEEngine(object):
+class MDPGapEEngine(TreeEngine):
     def __init__(self, env_kind, n_trees, n_actions, episodes, horizon, gamma, upper_bound, accuracy, confidence,
                  continuation_type="uniform", max_next_states_count=1, mdp=None, device="cuda"):
-        import torch
-        self.torch = torch
-        self.lib = _lib.load()
-        self.device = torch.device(device)
+        super(MDPGapEEngine, self).__init__(n_trees, _lib.MDP_GAPE_RESULT_WORDS, device)
+        torch = self.torch
         if env_kind not in (_lib.ENV_FINITE, _lib.ENV_HIGHWAY):
             raise NotImplementedError("MDP-GapE runs on finite MDPs and HighwayLite")
         if upper_bound["type"] != "kullback-leibler":
             # the reference only implements the KL bounds (mdp_gape.py:200-212); any other type leaves infinite
             # bounds whose backups are NaN
             raise NotImplementedError("MDP-GapE supports the kullback-leibler upper bound only")
-        self.n_trees, self.n_actions = int(n_trees), int(n_actions)
+        self.n_actions = int(n_actions)
         self.episodes, self.horizon = int(episodes), int(horizon)
         self.n_next = int(max_next_states_count)
         self.capacity = 1 + (self.episodes + 2) * self.horizon * (self.n_actions + self.n_next)
@@ -42,35 +41,25 @@ class MDPGapEEngine(object):
         self.transition_thresholds = table(upper_bound["transition_threshold"])
         self.init_upper = torch.as_tensor(init_upper, device=self.device)
         self.tables = FiniteTables(mdp, self.device) if env_kind == _lib.ENV_FINITE else None
-        shape = (self.n_trees, self.capacity)
-        for n in _lib.MDP_GAPE_TREE_FIELDS:
-            dtype = torch.int32 if n in ("parent", "first_child", "count", "meta") else torch.float64
-            setattr(self, n, torch.empty(shape, dtype=dtype, device=self.device))
+        self.tree = _lib.MDPGapETree(*self._alloc_tree(_lib.MDP_GAPE_TREE_FIELDS, self.capacity))
         self.cfg = _lib.MDPGapEConfig(env_kind, self.n_trees, self.n_actions, self.episodes, self.horizon,
                                       self.capacity, self.n_next, 1 if continuation_type == "uniform" else 0, gamma,
                                       float(accuracy), self.thresholds.data_ptr(),
                                       self.transition_thresholds.data_ptr(), self.init_upper.data_ptr(),
                                       self.tables.struct() if self.tables else _lib.FiniteMDP())
-        self.tree = _lib.MDPGapETree(*[getattr(self, n).data_ptr() for n in _lib.MDP_GAPE_TREE_FIELDS])
         self.plan_buf = torch.empty(self.n_trees, dtype=torch.int8, device=self.device)
-        self.result = torch.empty((self.n_trees, _lib.MDP_GAPE_RESULT_WORDS), dtype=torch.int32, device=self.device)
-        self.rng = torch.empty((self.n_trees, _lib.PCG64_STATE_WORDS), dtype=torch.int64, device=self.device)
 
     def plan(self, root_states, rng_words):
         """root_states: [n_trees] state ids (finite) or [n_trees, 136] words (HighwayLite), on the device."""
-        self.rng.copy_(self.torch.from_numpy(np.ascontiguousarray(rng_words).view(np.int64)))
+        self._load_rng(rng_words)
         _lib.check(self.lib.b2_mdp_gape_plan(self.cfg, _lib.ptr(root_states), self.tree, _lib.ptr(self.rng),
                                              _lib.ptr(self.plan_buf), _lib.ptr(self.result), _lib.current_stream()))
 
-    def finish(self):
-        """-> (plans: one [action] per tree, result words [n_trees, 8], PCG64 words after the search)."""
-        res = self.result.cpu().numpy()
+    def _check(self, res):
         if (res[:, 2] == 1).any():
             raise ValueError("This planner assumes that all rewards are normalized in [0, 1]")   # olop.py:133-134
         if (res[:, 2] == 2).any():
             raise ValueError("max() arg is an empty sequence")       # one available root action (mdp_gape.py:247)
-        plans = [[int(a)] for a in res[:, 3]]
-        return plans, res, self.rng.cpu().numpy().view(np.uint64)
 
     def tree_dict(self, tree=0):
         """Every node array of one tree, in creation order; `action` is the env action of a chance node, the
@@ -78,8 +67,6 @@ class MDPGapEEngine(object):
         n = int(self.result[tree, 0].item())
         out = {k: getattr(self, k)[tree, :n].cpu().numpy() for k in _lib.MDP_GAPE_TREE_FIELDS}
         meta = out["meta"]
-        action = (meta & 0xff).astype(int)
-        action[action == 0xff] = -1
-        out.update(action=action, n_children=(meta >> 8) & 0xff, done=((meta >> 16) & 1).astype(bool),
+        out.update(action=decode_action(meta), n_children=(meta >> 8) & 0xff, done=((meta >> 16) & 1).astype(bool),
                    kind=(meta >> 17) & 1, cumulative_reward=out["cumulative"])
         return out

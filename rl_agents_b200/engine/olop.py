@@ -5,6 +5,7 @@ import numpy as np
 
 from rl_agents_b200 import _lib
 from rl_agents_b200.engine.tables import FiniteTables
+from rl_agents_b200.engine.tree_engine import TreeEngine, decode_action
 
 logger = logging.getLogger(__name__)
 
@@ -24,14 +25,12 @@ def thresholds_for(upper_bound, episodes):
     return out
 
 
-class OLOPEngine(object):
+class OLOPEngine(TreeEngine):
     def __init__(self, env_kind, n_trees, n_actions, episodes, horizon, gamma, upper_bound, continuation_type="zeros",
                  mdp=None, device="cuda"):
-        import torch
-        self.torch = torch
-        self.lib = _lib.load()
-        self.device = torch.device(device)
-        self.n_trees, self.n_actions = int(n_trees), int(n_actions)
+        super(OLOPEngine, self).__init__(n_trees, _lib.OLOP_RESULT_WORDS, device)
+        torch = self.torch
+        self.n_actions = int(n_actions)
         self.episodes, self.horizon = int(episodes), int(horizon)
         self.capacity = 1 + self.episodes * self.horizon * self.n_actions
         self.kl = upper_bound["type"] == "kullback-leibler"
@@ -44,43 +43,32 @@ class OLOPEngine(object):
         self.thresholds = torch.as_tensor(thresholds_for(upper_bound, self.episodes) if self.kl
                                           else np.zeros(max(self.episodes, 1)), device=self.device)
         self.tables = FiniteTables(mdp, self.device) if env_kind == _lib.ENV_FINITE else None
-        shape = (self.n_trees, self.capacity)
-        i32, f64 = torch.int32, torch.float64
-        names = ("parent", "first_child", "count", "meta")
-        for n in names:
-            setattr(self, n, torch.empty(shape, dtype=i32, device=self.device))
-        for n in ("cumulative", "mu_ucb", "upper"):
-            setattr(self, n, torch.empty(shape, dtype=f64, device=self.device))
+        self.tree = _lib.OLOPTree(*self._alloc_tree(_lib.OLOP_TREE_FIELDS, self.capacity))
         self.cfg = _lib.OLOPConfig(env_kind, self.n_trees, self.n_actions, self.episodes, self.horizon, self.capacity,
                                    1 if self.kl else 0, 1 if continuation_type == "uniform" else 0, gamma,
                                    self.thresholds.data_ptr(), self.init_upper.data_ptr(),
                                    self.tables.struct() if self.tables else _lib.FiniteMDP())
-        self.tree = _lib.OLOPTree(*[getattr(self, n).data_ptr() for n in names + ("cumulative", "mu_ucb", "upper")])
         self.plan_buf = torch.empty((self.n_trees, max(self.horizon, 1)), dtype=torch.int8, device=self.device)
-        self.result = torch.empty((self.n_trees, _lib.OLOP_RESULT_WORDS), dtype=i32, device=self.device)
-        self.rng = torch.empty((self.n_trees, _lib.PCG64_STATE_WORDS), dtype=torch.int64, device=self.device)
 
     def plan(self, root_states, rng_words):
-        self.rng.copy_(self.torch.from_numpy(np.ascontiguousarray(rng_words).view(np.int64)))
+        self._load_rng(rng_words)
         _lib.check(self.lib.b2_olop_plan(self.cfg, _lib.ptr(root_states), self.tree, _lib.ptr(self.rng),
                                          _lib.ptr(self.plan_buf), _lib.ptr(self.result), _lib.current_stream()))
 
-    def finish(self):
-        res = self.result.cpu().numpy()
+    def _check(self, res):
         if (res[:, 2] == 1).any():
             raise ValueError("This planner assumes that all rewards are normalized in [0, 1]")   # olop.py:133-134
         if (res[:, 2] == 2).any():
             raise KeyError(0)                         # "zeros" continuation, action 0 unavailable (olop.py:82,88)
-        plans_dev = self.plan_buf.cpu().numpy()
-        plans = [plans_dev[i, :res[i, 1]].astype(int).tolist() for i in range(self.n_trees)]
-        return plans, res, self.rng.cpu().numpy().view(np.uint64)
+
+    def _plans(self, res):
+        plans = self.plan_buf.cpu().numpy()
+        return [plans[i, :res[i, 1]].astype(int).tolist() for i in range(self.n_trees)]
 
     def tree_dict(self, tree=0):
         n = int(self.result[tree, 0].item())
         meta = self.meta[tree, :n].cpu().numpy()
-        action = (meta & 0xff).astype(int)
-        action[action == 0xff] = -1
-        return {"parent": self.parent[tree, :n].cpu().numpy(), "action": action,
+        return {"parent": self.parent[tree, :n].cpu().numpy(), "action": decode_action(meta),
                 "count": self.count[tree, :n].cpu().numpy(), "done": ((meta >> 16) & 1).astype(bool),
                 "cumulative_reward": self.cumulative[tree, :n].cpu().numpy(),
                 "mu_ucb": self.mu_ucb[tree, :n].cpu().numpy(), "upper": self.upper[tree, :n].cpu().numpy()}

@@ -5,6 +5,7 @@ import numpy as np
 
 from rl_agents_b200 import _lib
 from rl_agents_b200.engine.tables import FiniteTables, gamma_tables, terminal_bonus_table
+from rl_agents_b200.engine.tree_engine import decode_action
 
 logger = logging.getLogger(__name__)
 
@@ -101,9 +102,7 @@ class OPDEngine(object):
         """Host copy of one tree in the layout of the oracle / golden dumps."""
         n = int(self.result[tree, 0].item())
         meta = self.meta[tree, :n].cpu().numpy()
-        action = (meta & 0xff).astype(int)
-        action[action == 0xff] = -1
-        return {"parent": self.parent[tree, :n].cpu().numpy(), "action": action,
+        return {"parent": self.parent[tree, :n].cpu().numpy(), "action": decode_action(meta),
                 "count": self.count[tree, :n].cpu().numpy(), "depth": self.depth[tree, :n].cpu().numpy(),
                 "first_child": self.first_child[tree, :n].cpu().numpy(), "n_children": (meta >> 8) & 0xff,
                 "done": ((meta >> 16) & 1).astype(bool), "reward": self.reward[tree, :n].cpu().numpy(),

@@ -3,6 +3,7 @@ import numpy as np
 
 from rl_agents_b200 import _lib
 from rl_agents_b200.engine.tables import SampledFiniteTables
+from rl_agents_b200.engine.tree_engine import TreeEngine
 
 # what the reference raises at horizon 0: the root has no children, and selection_rule's np.amax of its empty value
 # list fails (sparse_sampling.py:45-46, :53-56; abstract.py:301)
@@ -28,19 +29,17 @@ def worst_case_nodes(n_actions, horizon, C):
     return sum(b ** d for d in range(horizon + 1)) + n_actions * sum(b ** d for d in range(horizon))
 
 
-class SparseSamplingEngine(object):
+class SparseSamplingEngine(TreeEngine):
     def __init__(self, env_kind, n_trees, n_actions, horizon, C, gamma, mdp=None, record_tree=False, capacity=None,
                  device="cuda"):
         """record_tree: also dump every tree in creation order (capacity: nodes per tree, by default the worst
         case).  The plan itself needs no node storage."""
-        import torch
-        self.torch = torch
-        self.lib = _lib.load()
-        self.device = torch.device(device)
+        super(SparseSamplingEngine, self).__init__(n_trees, _lib.SPARSE_SAMPLING_RESULT_WORDS, device)
+        torch = self.torch
         if env_kind not in (_lib.ENV_FINITE, _lib.ENV_HIGHWAY):
             raise NotImplementedError("sparse sampling runs on finite MDPs and HighwayLite")
         self.env_kind = env_kind
-        self.n_trees, self.n_actions = int(n_trees), int(n_actions)
+        self.n_actions = int(n_actions)
         self.horizon, self.C, self.gamma = int(horizon), int(C), float(gamma)
         check_horizon_and_c(self.horizon, self.C)
         self.tables = SampledFiniteTables(mdp, self.device) if env_kind == _lib.ENV_FINITE else None
@@ -54,29 +53,21 @@ class SparseSamplingEngine(object):
                                                                                         self.C)
             if self.capacity >= 2 ** 31:
                 raise ValueError("a recorded tree of up to %d nodes does not fit int32 node ids" % self.capacity)
-            shape = (self.n_trees, self.capacity)
-            for n in _lib.SPARSE_SAMPLING_TREE_FIELDS:
-                setattr(self, n, torch.empty(shape, dtype=torch.float64 if n == "value" else torch.int32,
-                                             device=self.device))
             self.tree = _lib.SparseSamplingTree(self.capacity, 0,
-                                                *[getattr(self, n).data_ptr() for n in _lib.SPARSE_SAMPLING_TREE_FIELDS])
+                                                *self._alloc_tree(_lib.SPARSE_SAMPLING_TREE_FIELDS, self.capacity))
         self.root_q = torch.empty((self.n_trees, self.n_actions), dtype=torch.float64, device=self.device)
         self.plan_buf = torch.empty(self.n_trees, dtype=torch.int8, device=self.device)
-        self.result = torch.empty((self.n_trees, _lib.SPARSE_SAMPLING_RESULT_WORDS), dtype=torch.int32,
-                                  device=self.device)
-        self.rng = torch.empty((self.n_trees, _lib.PCG64_STATE_WORDS), dtype=torch.int64, device=self.device)
 
     def plan(self, root_states, rng_words):
         """root_states: [n_trees] state ids (finite) or [n_trees, 136] words (HighwayLite), on the device."""
-        self.rng.copy_(self.torch.from_numpy(np.ascontiguousarray(rng_words).view(np.int64)))
+        self._load_rng(rng_words)
         _lib.check(self.lib.b2_sparse_sampling_plan(self.cfg, _lib.ptr(root_states), self.tree, _lib.ptr(self.workspace),
                                                     _lib.ptr(self.rng), _lib.ptr(self.root_q), _lib.ptr(self.plan_buf),
                                                     _lib.ptr(self.result), _lib.current_stream()))
 
-    def finish(self):
-        """-> (plans: one [action] per tree, result words [n_trees, 8], PCG64 words after the search).  A sampled
-        probability row that Generator.choice rejects raises its ValueError, as the reference's env step does."""
-        res = self.result.cpu().numpy()
+    def _check(self, res):
+        """A sampled probability row that Generator.choice rejects raises its ValueError, as the reference's env step
+        does."""
         bad = np.nonzero(res[:, 4] == 2)[0]
         if bad.size:
             p = self.tables.row(int(res[bad[0], 5]))
@@ -84,8 +75,6 @@ class SparseSamplingEngine(object):
             raise AssertionError("row %d was flagged but Generator.choice accepts it" % int(res[bad[0], 5]))
         if (res[:, 4] != 0).any():
             raise RuntimeError("sparse-sampling tree dump exhausted its capacity of %d nodes" % self.capacity)
-        plans = [[int(a)] for a in res[:, 3]]
-        return plans, res, self.rng.cpu().numpy().view(np.uint64)
 
     def tree_dict(self, tree=0):
         """The dump of one tree in creation order: parent, kind (0 decision, 1 chance), key, depth, count, value."""
