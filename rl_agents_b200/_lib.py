@@ -75,13 +75,18 @@ class GBOPDConfig(ctypes.Structure):
                 ("accuracy", c_double), ("mdp", FiniteMDP), ("rev_ptr", c_void_p), ("rev_idx", c_void_p)]
 
 
+GBOP_TREE_FIELDS = ("parent", "first_child", "depth", "count", "meta", "reward", "lower", "obs")
+
+
 class GBOPTree(ctypes.Structure):
-    _fields_ = [(n, c_void_p) for n in ("parent", "first_child", "depth", "count", "meta", "reward", "lower", "obs")]
+    _fields_ = [(n, c_void_p) for n in GBOP_TREE_FIELDS]
+
+
+OPD_TREE_FIELDS = ("parent", "first_child", "depth", "count", "meta", "reward", "lower", "upper")
 
 
 class OPDTree(ctypes.Structure):
-    _fields_ = [(n, c_void_p) for n in ("parent", "first_child", "depth", "count", "meta", "reward",
-                                        "lower", "upper", "state")]
+    _fields_ = [(n, c_void_p) for n in OPD_TREE_FIELDS + ("state",)]
 
 
 class OPDHostConfig(ctypes.Structure):

@@ -24,7 +24,6 @@ class DiscreteRobustPlanner(AbstractPlanner):
 
     def plan(self, state, observation):
         """state: the list of the M model envs (what JointEnv holds as joint_state)."""
-        import torch
         from rl_agents_b200.engine.opd import OPDWaveEngine
         models = list(state)
         descs = [describe(m) for m in models]
@@ -40,11 +39,7 @@ class DiscreteRobustPlanner(AbstractPlanner):
                                                             self.config.get("terminal_reward", 0), n_models=len(models),
                                                             model_mdps=[d.mdp for d in descs] if d0.mdp is not None
                                                             else None))
-        root = torch.from_numpy(np.ascontiguousarray(np.stack([d.root.reshape(-1) for d in descs]))).to(eng.device)
-        eng.plan(root.contiguous())
-        plans, _ = eng.finish([self.np_random])
-        self.last_tree = eng
-        return plans[0]
+        return self.search_host_ties(eng, np.stack([d.root.reshape(-1) for d in descs]))
 
 
 @register_with_reference

@@ -166,6 +166,15 @@ class AbstractPlanner(Configurable):
         self.last_tree = engine
         return plans[0], res[0]
 
+    def search_host_ties(self, engine, root):
+        """One tree from `root` (int32 host array: the root's state id or words; DROP: one row per model) on a
+        value-bound engine, which completes its plan past a tie with the planner's generator -> the plan."""
+        import torch
+        engine.plan(torch.from_numpy(root).to(engine.device).contiguous())
+        plans, _ = engine.finish([self.np_random])
+        self.last_tree = engine
+        return plans[0]
+
     def get_visits(self):
         return defaultdict(int)
 

@@ -62,14 +62,8 @@ class OptimisticDeterministicPlanner(AbstractPlanner):
         return self.cached_engine(key, make)
 
     def plan(self, state, observation):
-        import torch
         d = describe(state)
-        eng = self._engine_for(d)
-        root = torch.from_numpy(d.root.reshape(1, -1) if d.root.size > 1 else d.root).to(eng.device)
-        eng.plan(root.contiguous())
-        plans, res = eng.finish([self.np_random])
-        self.last_tree = eng
-        return plans[0]
+        return self.search_host_ties(self._engine_for(d), d.root)
 
 
 @register_with_reference

@@ -20,7 +20,6 @@ class StateAwarePlanner(AbstractPlanner):
         return cfg
 
     def plan(self, state, observation):
-        import torch
         from rl_agents_b200.engine.gbop import GBOPEngine
         d = describe(state)
         if d.kind != _lib.ENV_FINITE:
@@ -32,11 +31,9 @@ class StateAwarePlanner(AbstractPlanner):
                                                          d.mdp, self.config.get("terminal_reward", 0),
                                                          self.config["backup_aggregated_nodes"],
                                                          self.config["prune_suboptimal_leaves"], self.config["accuracy"]))
-        eng.plan(torch.from_numpy(d.root).to(eng.device).contiguous())
-        plans, _ = eng.finish([self.np_random])
-        self.last_tree = eng
+        plan = self.search_host_ties(eng, d.root)
         self.state_values = eng.state_values(0)
-        return plans[0]
+        return plan
 
 
 @register_with_reference

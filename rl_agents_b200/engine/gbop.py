@@ -2,88 +2,42 @@
 import numpy as np
 
 from rl_agents_b200 import _lib
-from rl_agents_b200.engine.tables import FiniteTables, gamma_tables, terminal_bonus_table
-from rl_agents_b200.engine.tree_engine import decode_action
+from rl_agents_b200.engine.tables import FiniteTables
+from rl_agents_b200.engine.tree_engine import HostTieEngine, TreeEngine, decode_action
 
 
-class GBOPEngine(object):
+class GBOPEngine(HostTieEngine):
     """n_trees independent GBOP-T decisions per launch (one warp per tree) on a deterministic finite MDP."""
+    # StateAwarePlanner.plan runs get_plan() twice (state_aware.py:124, :130; the first inside super().plan()): a tie
+    # consumes the planner RNG on both walks, the second is returned
+    TIE_WALKS = 2
 
     def __init__(self, n_trees, n_actions, budget, gamma, mdp, terminal_reward=0.0, backup_aggregated_nodes=True,
                  prune_suboptimal_leaves=True, accuracy=0, device="cuda", queue_factor=64):
-        import torch
-        self.torch = torch
-        self.lib = _lib.load()
-        self.device = torch.device(device)
-        self.n_trees, self.n_actions = int(n_trees), int(n_actions)
-        self.n_expansions = int(budget) // self.n_actions
-        self.capacity = 1 + self.n_expansions * self.n_actions
-        self.plan_capacity = self.n_expansions + 1
+        super(GBOPEngine, self).__init__(n_trees, n_actions, budget, gamma, terminal_reward, device)
         gamma = float(gamma)
-        gp, _ = gamma_tables(gamma, self.n_expansions + 2)
-        self.gamma_pow = torch.as_tensor(gp, device=self.device)
-        self.terminal_bonus = torch.as_tensor(terminal_bonus_table(terminal_reward, gamma, self.n_expansions + 2),
-                                              device=self.device)
         self.tables = FiniteTables(mdp, self.device)
         self.n_states = self.tables.n_states
-        shape = (self.n_trees, self.capacity)
-        i32, f64 = torch.int32, torch.float64
-        names_i = ("parent", "first_child", "depth", "count", "meta", "obs")
-        for n in names_i:
-            setattr(self, n, torch.empty(shape, dtype=i32, device=self.device))
-        self.reward = torch.empty(shape, dtype=f64, device=self.device)
-        self.lower = torch.empty(shape, dtype=f64, device=self.device)
         self.cfg = _lib.GBOPConfig(self.n_trees, self.n_actions, self.n_expansions, self.capacity, self.plan_capacity,
                                    int(queue_factor) * self.capacity, 1 if backup_aggregated_nodes else 0,
                                    1 if prune_suboptimal_leaves else 0, gamma, 1 / (1 - gamma), accuracy * (1 - gamma),
                                    self.gamma_pow.data_ptr(), self.terminal_bonus.data_ptr(), self.tables.struct())
-        self.tree = _lib.GBOPTree(*[t.data_ptr() for t in (self.parent, self.first_child, self.depth, self.count, self.meta,
-                                                           self.reward, self.lower, self.obs)])
+        self.tree = _lib.GBOPTree(*self._alloc_tree(_lib.GBOP_TREE_FIELDS, self.capacity))
         ws = self.lib.b2_gbop_workspace_bytes(self.cfg)
         if ws < 0:
             raise _lib.B2Error("unsupported GBOP configuration")
         self.ws_per_tree = int(ws) // self.n_trees
-        self.workspace = torch.empty(int(ws), dtype=torch.uint8, device=self.device)
-        self.plan_buf = torch.empty((self.n_trees, self.plan_capacity), dtype=torch.int8, device=self.device)
-        self.result = torch.empty((self.n_trees, _lib.OPD_RESULT_WORDS), dtype=i32, device=self.device)
+        self.workspace = self.torch.empty(int(ws), dtype=self.torch.uint8, device=self.device)
 
     def plan(self, root_states):
         assert root_states.dtype == self.torch.int32 and root_states.is_cuda and root_states.is_contiguous()
         _lib.check(self.lib.b2_gbop_plan(self.cfg, _lib.ptr(root_states), self.tree, _lib.ptr(self.workspace),
                                          _lib.ptr(self.plan_buf), _lib.ptr(self.result), _lib.current_stream()))
 
-    def finish(self, np_randoms=None):
-        """Synchronise; returns (plans, result).  StateAwarePlanner.plan runs get_plan() twice (state_aware.py:124,
-        :130; the first inside super().plan()): a tie consumes the planner RNG on both walks, the second is returned."""
-        res = self.result.cpu().numpy()
-        if (res[:, 4] != 0).any():
-            raise ValueError("This planner assumes that all rewards are normalized in [0, 1]")
+    def _check(self, res):
+        super(GBOPEngine, self)._check(res)
         if (res[:, 7] != 0).any():
             raise _lib.B2Error("GBOP backup queue overflow: raise queue_factor")
-        plans_dev = self.plan_buf.cpu().numpy()
-        plans = []
-        for i in range(self.n_trees):
-            head = plans_dev[i, :res[i, 5]].astype(int).tolist()
-            if res[i, 6] >= 0:
-                rng = np_randoms[i] if np_randoms is not None else np.random.default_rng()
-                self._host_plan_from(i, int(res[i, 6]), rng)
-                plans.append(head + self._host_plan_from(i, int(res[i, 6]), rng))
-            else:
-                plans.append(head)
-        return plans, res
-
-    def _host_plan_from(self, tree, node, rng):
-        fc = self.first_child[tree].cpu().numpy()
-        meta = self.meta[tree].cpu().numpy()
-        lower = self.lower[tree].cpu().numpy()
-        plan = []
-        while fc[node] >= 0:
-            n = (meta[node] >> 8) & 0xff
-            x = lower[fc[node]:fc[node] + n]
-            indices = np.nonzero(x == np.amax(x))[0]
-            node = fc[node] + int(rng.choice(indices))
-            plan.append(int(meta[node] & 0xff))
-        return plan
 
     def state_values(self, tree=0):
         off = tree * self.ws_per_tree
@@ -100,16 +54,14 @@ class GBOPEngine(object):
                 "obs": self.obs[tree, :n].cpu().numpy()}
 
 
-class GBOPDEngine(object):
+class GBOPDEngine(TreeEngine):
     """n_trees independent GBOP-D decisions per launch (GraphBasedPlanner, one warp per decision)."""
 
     def __init__(self, n_trees, n_actions, budget, gamma, mdp, accuracy=1e-2, sampling_timeout=100, device="cuda",
                  queue_factor=256):
-        import torch
-        self.torch = torch
-        self.lib = _lib.load()
-        self.device = torch.device(device)
-        self.n_trees, self.n_actions = int(n_trees), int(n_actions)
+        super(GBOPDEngine, self).__init__(n_trees, _lib.OPD_RESULT_WORDS, device)
+        torch = self.torch
+        self.n_actions = int(n_actions)
         self.tables = FiniteTables(mdp, self.device)
         S = self.n_states = self.tables.n_states
         T = np.asarray(mdp.transition, dtype=np.int64)
@@ -129,23 +81,22 @@ class GBOPDEngine(object):
         self.upper = torch.empty((self.n_trees, S), dtype=torch.float64, device=self.device)
         self.flags = torch.empty((self.n_trees, S), dtype=torch.uint8, device=self.device)
         self.queue = torch.empty((self.n_trees, self.queue_capacity), dtype=torch.int32, device=self.device)
-        self.rng = torch.empty((self.n_trees, _lib.PCG64_STATE_WORDS), dtype=torch.int64, device=self.device)
         self.plan_buf = torch.empty((self.n_trees, self.timeout), dtype=torch.int8, device=self.device)
-        self.result = torch.empty((self.n_trees, _lib.OPD_RESULT_WORDS), dtype=torch.int32, device=self.device)
 
     def plan(self, root_states, rng_words):
-        self.rng.copy_(self.torch.from_numpy(np.ascontiguousarray(rng_words).view(np.int64)))
+        self._load_rng(rng_words)
         _lib.check(self.lib.b2_gbopd_plan(self.cfg, _lib.ptr(root_states), _lib.ptr(self.lower), _lib.ptr(self.upper),
                                           _lib.ptr(self.flags), _lib.ptr(self.queue), _lib.ptr(self.rng),
                                           _lib.ptr(self.plan_buf), _lib.ptr(self.result), _lib.current_stream()))
 
-    def finish(self):
-        res = self.result.cpu().numpy()
+    def _check(self, res):
         if (res[:, 7] != 0).any():
             raise _lib.B2Error("GBOP-D backup queue overflow: raise queue_factor")
+
+    def _plans(self, res):
+        """The plan words up to result word 5."""
         plans_dev = self.plan_buf.cpu().numpy()
-        return [plans_dev[i, :res[i, 5]].astype(int).tolist() for i in range(self.n_trees)], res, \
-            self.rng.cpu().numpy().view(np.uint64)
+        return [plans_dev[i, :res[i, 5]].astype(int).tolist() for i in range(self.n_trees)]
 
     def nodes(self, tree=0):
         fl = self.flags[tree].cpu().numpy()
