@@ -633,6 +633,67 @@ int b2_sparse_sampling_plan(const b2_sparse_sampling_config* cfg, const int32_t*
                             const b2_sparse_sampling_tree* tree, void* workspace, uint64_t* rng, double* root_q,
                             int8_t* plan, int32_t* result, void* stream);
 
+/* ------------------------------------------------------------------------
+ * MCTS with double progressive widening -- rl_agents/agents/tree_search/mcts_dpw.py (MCTSDPW).  Finite MDPs in all
+ * three modes (the env copy's `seed(np_random.randint(2**30))` once per run, then Generator.choice(p.size, p=p) per
+ * step, replayed on the device) and HighwayLite.  Widening thresholds and the exploration bonus come from host tables
+ * built with the reference's own expressions, so every node equals the reference's bit for bit.
+ * ---------------------------------------------------------------------- */
+typedef struct b2_mcts_dpw_config {
+    int32_t env_kind;        /* B2_ENV_FINITE or B2_ENV_HIGHWAY                                                 */
+    int32_t n_trees;
+    int32_t n_actions;       /* 1..8; finite: every action is available; HighwayLite: 5                         */
+    int32_t episodes;        /* config["episodes"] >= 1: runs per tree (mcts.py:179-184)                         */
+    int32_t horizon;         /* config["horizon"] >= 1                                                          */
+    int32_t node_capacity;   /* per tree, >= 1 + 2 * episodes (a run adds at most a chance and a decision node)  */
+    int32_t rollout_policy;  /* 0 random_available, 1 random, 2 preference (mcts.py:46-97), as b2_mcts_config    */
+    int32_t rollout_pref_action;
+    int32_t closed_loop;     /* config["closed_loop"]: key a chance node's children on the observation (:79)     */
+    int32_t open_key;        /* the key of every observation in open loop: sha1("None")[:5] as a 20-bit integer  */
+    int32_t env_draws;       /* finite: 1 when the MDP is not "deterministic" (every step draws from the env's own
+                                generator, a width-1 row included)                                             */
+    int32_t reserved;
+    double temperature;      /* config["temperature"]: UCB index value + temperature * bonus (:150)              */
+    const double* gamma_pow; /* [horizon] gamma**d (host Python floats)                                          */
+    const double* uniform_cdf;   /* [(n_actions+1), n_actions], as b2_mcts_config                               */
+    const double* pref_cdf;      /* [(n_actions+1), (n_actions+1), n_actions], read when rollout_policy == 2     */
+    const int32_t* action_widen; /* [episodes+1] by decision-node count N: the largest m <= n_actions for which
+                                    `k_action*N**alpha_action < m` is false (-1: none); a node with m children
+                                    adds an action iff m <= action_widen[N] and not every action has one (:121-127) */
+    const int32_t* state_widen;  /* [episodes+1] the same for k_state / alpha_state, m <= episodes (:175)        */
+    const double* bonus;         /* [episodes*(episodes+1)/2] np.sqrt(np.log(N / n)) at N (N-1)/2 + n-1,
+                                    1 <= n <= N <= episodes (host numpy)                                        */
+    const int32_t* obs_keys;     /* finite, closed loop: [S] sha1(str(s))[:5] as a 20-bit integer                 */
+    const uint8_t* terminal;     /* finite: [S], `done` of a step taken in s                                      */
+    b2_finite_mdp_sampled mdp;   /* env_kind == FINITE                                                          */
+} b2_mcts_dpw_config;
+
+/* One arena for decision and chance nodes; node id = creation order.  A node's children form a list first_child ->
+ * next_sibling -> ... in creation order (the reference's dict order). */
+typedef struct b2_mcts_dpw_tree {
+    int32_t* parent;         /* -1 for the root                                                                  */
+    int32_t* first_child;
+    int32_t* next_sibling;   /* -1 at the end of a list                                                          */
+    int32_t* count;          /* Node.count                                                                       */
+    int32_t* kind;           /* 0 DecisionNode, 1 ChanceNode                                                     */
+    int32_t* key;            /* chance: the action; decision: the observation key (closed loop: obs_keys[s] on a
+                                finite MDP, the step count t on HighwayLite; open loop: open_key), -1 at the root */
+    double* value;           /* MCTSNode.value (mcts.py:248-255)                                                 */
+} b2_mcts_dpw_tree;
+
+#define B2_MCTS_DPW_RESULT_WORDS 8
+/* per tree int32 result: [0] n_nodes [1] runs completed [2] env steps [3] recommended action (-1 on error)
+ * [4] error (1: node_capacity exhausted; 2: a sampled probability row that Generator.choice rejects; 3: a decision
+ * node that can neither add an action nor select one; 4: a chance node that can neither add a state nor choose one)
+ * [5] the rejected row, s * n_actions + a (-1 otherwise) */
+
+/* MCTSDPW.plan (mcts.py:179-184, mcts_dpw.py:59-94) for n_trees independent decisions, one tree per lane (finite) or
+ * per 16-lane group (HighwayLite), runs in strict order.  rng: uint64 [n_trees, 6] numpy PCG64 states of the planners'
+ * streams, advanced in place; root_states: [n_trees] state ids or [n_trees, 136] words; plan: int8 [n_trees], the
+ * root's selection_rule (mcts.py:212-218). */
+int b2_mcts_dpw_plan(const b2_mcts_dpw_config* cfg, const int32_t* root_states, const b2_mcts_dpw_tree* tree,
+                     uint64_t* rng, int8_t* plan, int32_t* result, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -22,6 +22,7 @@ OLOP_RESULT_WORDS = 8
 MDP_GAPE_RESULT_WORDS = 8
 BRUE_RESULT_WORDS = 8
 SPARSE_SAMPLING_RESULT_WORDS = 8
+MCTS_DPW_RESULT_WORDS = 8
 PCG64_STATE_WORDS = 6
 
 
@@ -179,6 +180,23 @@ class SparseSamplingTree(ctypes.Structure):
     _fields_ = [("capacity", c_int32), ("reserved", c_int32)] + [(n, c_void_p) for n in SPARSE_SAMPLING_TREE_FIELDS]
 
 
+class MCTSDPWConfig(ctypes.Structure):
+    _fields_ = [("env_kind", c_int32), ("n_trees", c_int32), ("n_actions", c_int32), ("episodes", c_int32),
+                ("horizon", c_int32), ("node_capacity", c_int32), ("rollout_policy", c_int32),
+                ("rollout_pref_action", c_int32), ("closed_loop", c_int32), ("open_key", c_int32),
+                ("env_draws", c_int32), ("reserved", c_int32), ("temperature", c_double), ("gamma_pow", c_void_p),
+                ("uniform_cdf", c_void_p), ("pref_cdf", c_void_p), ("action_widen", c_void_p),
+                ("state_widen", c_void_p), ("bonus", c_void_p), ("obs_keys", c_void_p), ("terminal", c_void_p),
+                ("mdp", FiniteMDPSampled)]
+
+
+MCTS_DPW_TREE_FIELDS = ("parent", "first_child", "next_sibling", "count", "kind", "key", "value")
+
+
+class MCTSDPWTree(ctypes.Structure):
+    _fields_ = [(n, c_void_p) for n in MCTS_DPW_TREE_FIELDS]
+
+
 EXPORTS = {
     "b2_last_error": (ctypes.c_char_p, []),
     "b2_version": (c_int, []),
@@ -231,6 +249,8 @@ EXPORTS = {
     "b2_sparse_sampling_workspace_bytes": (c_int64, [ctypes.POINTER(SparseSamplingConfig)]),
     "b2_sparse_sampling_plan": (c_int, [ctypes.POINTER(SparseSamplingConfig), c_void_p,
                                         ctypes.POINTER(SparseSamplingTree)] + [c_void_p] * 6),
+    "b2_mcts_dpw_plan": (c_int, [ctypes.POINTER(MCTSDPWConfig), c_void_p, ctypes.POINTER(MCTSDPWTree), c_void_p,
+                                 c_void_p, c_void_p, c_void_p]),
 }
 
 _lib = None

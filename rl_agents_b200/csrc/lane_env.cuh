@@ -5,11 +5,34 @@
 //
 // step() reports truncation separately; MCTS reads it, the other planners pass a dummy (the reference's 4-tuple step
 // drops truncation).
+//
+// The planners that sample stochastic finite MDPs draw from a b2_finite_mdp_sampled row with searchsorted_right()
+// (sparse_sampling.cu, which seeds a fresh env generator per sample) or step it with sampled_next() (mcts_dpw.cu).
 #pragma once
 #include "common.cuh"
 #include "highway_lite.cuh"
+#include "pcg64.cuh"
 
 namespace b2 {
+
+// searchsorted(cdf, u, side="right") on a non-decreasing row: the number of entries <= u
+__device__ __forceinline__ int searchsorted_right(const double* cdf, int n, double u) {
+    int lo = 0, hi = n;
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (cdf[mid] <= u) lo = mid + 1; else hi = mid;
+    }
+    return lo;
+}
+
+// The next state of FiniteMDPEnv.step on row s * n_actions + a: next[row, k] with k = Generator.choice(p.size, p=p)
+// of the env's generator `env_rng`, i.e. searchsorted(cdf[row], random(), "right"); draw = false (a deterministic
+// table) takes k = 0 and leaves env_rng alone.  The caller checks row_ok first.
+__device__ __forceinline__ int sampled_next(const b2_finite_mdp_sampled& m, int64_t row, bool draw, Pcg64& env_rng) {
+    const int B = m.n_next;
+    const int k = draw ? searchsorted_right(m.cdf + row * B, B, env_rng.random()) : 0;
+    return m.next[row * B + k];
+}
 
 struct FiniteEnv {
     static constexpr int GROUP = 1;

@@ -25,6 +25,7 @@
 
 #include "common.cuh"
 #include "highway_lite.cuh"
+#include "lane_env.cuh"
 #include "pcg64.cuh"
 
 namespace b2 {
@@ -77,16 +78,6 @@ __device__ __forceinline__ void put(const b2_sparse_sampling_tree& tr, int64_t n
                                     int depth) {
     tr.parent[nb + id] = parent; tr.kind[nb + id] = kind; tr.key[nb + id] = key; tr.depth[nb + id] = depth;
     tr.count[nb + id] = 0; tr.value[nb + id] = 0.0;
-}
-
-// searchsorted(cdf, u, side="right") on a non-decreasing row: the number of entries <= u
-__device__ __forceinline__ int searchsorted_right(const double* cdf, int n, double u) {
-    int lo = 0, hi = n;
-    while (lo < hi) {
-        const int mid = (lo + hi) >> 1;
-        if (cdf[mid] <= u) lo = mid + 1; else hi = mid;
-    }
-    return lo;
 }
 
 struct SFiniteEnv {

@@ -17,8 +17,8 @@ def _np_random(seed):
 def run_batched_episodes(planner, seeds, budget, gamma, max_steps=40, device="cuda", planner_seed=0, **kw):
     """planner: "opd" | "mcts" | "olop" | "mdp_gape" (keywords: MDPGapEAgent config keys) | "brue" (keywords: BRUEAgent
     config keys) | "sparse_sampling" (keywords `horizon` and `C`, required as in SparseSamplingAgent's config; `budget`
-    is unused) | "vi" (ValueIterationAgent on the scenes' TTC-grid MDPs, `budget` = its `iterations`).  Every
-    episode: scene make_scene(seed), replanning at every step (receding_horizon 1, step_strategy reset -- the reference
+    is unused) | "mcts_dpw" (keywords: MCTSDPWAgent config keys) | "vi" (ValueIterationAgent on the scenes' TTC-grid
+    MDPs, `budget` = its `iterations`).  Every episode: scene make_scene(seed), replanning at every step (receding_horizon 1, step_strategy reset -- the reference
     defaults), until crash or `max_steps`.
     Returns dict(returns, lengths, crashed, decision_ms)."""
     import torch
@@ -64,6 +64,19 @@ def run_batched_episodes(planner, seeds, budget, gamma, max_steps=40, device="cu
     elif planner == "sparse_sampling":
         from rl_agents_b200.engine.sparse_sampling import SparseSamplingEngine
         eng = SparseSamplingEngine(_lib.ENV_HIGHWAY, n, 5, kw["horizon"], kw["C"], gamma, device=dev)
+    elif planner == "mcts_dpw":
+        # MCTSDPWAgent's completed planner config (mcts_dpw.py:20-54) with budget / gamma and any keyword overriding it
+        from rl_agents_b200.agents.tree_search.mcts_dpw import MCTSDPW, MCTSDPWAgent
+        from rl_agents_b200.engine.mcts_dpw import MCTSDPWEngine
+        cfg = MCTSDPWAgent.default_config()
+        MCTSDPWAgent.rec_update(cfg, dict(kw, budget=budget, gamma=gamma))
+        pcfg = MCTSDPW.default_config()
+        MCTSDPW.rec_update(pcfg, cfg)
+        episodes, horizon = (pcfg["episodes"], pcfg["horizon"]) if pcfg["horizon"] else allocation(budget, gamma)
+        eng = MCTSDPWEngine(_lib.ENV_HIGHWAY, n, 5, episodes, horizon, gamma, pcfg["temperature"], pcfg["k_action"],
+                            pcfg["alpha_action"], pcfg["k_state"], pcfg["alpha_state"],
+                            closed_loop=pcfg["closed_loop"],
+                            rollout_policy=MCTSDPWAgent.policy_factory(pcfg["rollout_policy"]), device=dev)
     elif planner == "vi":
         from rl_agents_b200.engine.ttc_vi import HighwayTTCVI
         eng = HighwayTTCVI(gamma, budget, device=dev)
