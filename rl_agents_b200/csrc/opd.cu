@@ -744,8 +744,9 @@ __global__ void __launch_bounds__(128) highway_step_kernel(int32_t* states, cons
 // Exhaustive check of hw::div_const against the IEEE division for the two constant divisors of the spec:
 // every fp32 mantissa, both signs, exponents -60 .. +60 (quotients stay normal); and of hw::div_fast against the
 // `/` operator on 2^33 operand pairs (every numerator mantissa x 1024 hashed divisors of either sign, both
-// magnitudes in 2^-40 .. 2^40); and of hw::sqrt_fast against sqrtf on every value of [2^-3, 2).  Counts mismatching
-// bit patterns.
+// magnitudes in 2^-40 .. 2^40), and of hw::div_nz on the same pairs and on zero numerators of either sign; and of
+// hw::sqrt_fast against sqrtf on every value of [2^-3, 2); and of hw::lane_of against clip(rint(y / 4), 0, 3) on every
+// fp32 bit pattern.  Counts mismatching bit patterns.
 __global__ void const_division_selftest_kernel(unsigned long long* mismatches) {
     const unsigned m = blockIdx.x * blockDim.x + threadIdx.x;       // mantissa, 2^23 threads
     unsigned long long bad = 0;
@@ -762,6 +763,11 @@ __global__ void const_division_selftest_kernel(unsigned long long* mismatches) {
         asm volatile("" : "+f"(x));
         bad += __float_as_uint(sqrtf(x)) != __float_as_uint(hw::sqrt_fast(x));
     }
+    for (unsigned hi = 0; hi < 512; ++hi) {      // hw::lane_of on all 2^32 bit patterns (NaN and +-inf included)
+        float y = __uint_as_float((hi << 23) | m);
+        asm volatile("" : "+f"(y));
+        bad += (int)fminf(fmaxf(rintf(y / hw::LANE_W), 0.0f), 3.0f) != hw::lane_of(y);
+    }
     unsigned long long h = 0x9e3779b97f4a7c15ull * (m + 1);
     for (int it = 0; it < 1024; ++it) {
         h ^= h >> 30; h *= 0xbf58476d1ce4e5b9ull; h ^= h >> 27; h *= 0x94d049bb133111ebull; h ^= h >> 31;
@@ -771,6 +777,9 @@ __global__ void const_division_selftest_kernel(unsigned long long* mismatches) {
         asm volatile("" : "+f"(y));      // opaque: the reference quotient below is the compiler's own division
         const float q = x / y, f = hw::div_fast(x, y);
         bad += __float_as_uint(q) != __float_as_uint(f);
+        bad += __float_as_uint(q) != __float_as_uint(hw::div_nz(x, y));
+        const float z = __uint_as_float(((unsigned)(h >> 45) & 1u) << 31);     // +0 or -0
+        bad += __float_as_uint(z / y) != __float_as_uint(hw::div_nz(z, y));
     }
     if (bad) atomicAdd(mismatches, bad);
 }
