@@ -3,7 +3,7 @@
 Compiles csrc/opd.cu to a cubin with the library's own nvcc flags (rl_agents_b200/build.py), disassembles it with
 inline line information and counts, per issue pipe, the instructions whose source position inside `hw::step` lies in
 the sub-step loop -- including what helpers inlined there (not_zero, idm_front, asin_p, ...) compiled to.  The scan
-path (exact x ties), the rank recount (after an overtake) and the collision loop are reported apart from the common
+path (exact x ties), the rank recount (first sub-step, and after an overtake) and the collision loop are reported apart from the common
 path.  CPU only: needs nvcc and nvdisasm, no GPU.
 
     python benchmarks/sass_census.py [--ops]

@@ -70,7 +70,6 @@ __device__ double estimate(const b2_brue_tree& tr, int64_t nb, int node, int lev
 template <class Env>
 __global__ void __launch_bounds__(128, 8) brue_kernel(BrueArgs a) {
     constexpr int G = Env::GROUP;
-    __shared__ float scratch[G == 16 ? 128 / 16 : 1][hw::SCRATCH_FLOATS];
     const int gtid = blockIdx.x * 128 + threadIdx.x;
     const int tree = gtid / G, li = gtid % G;
     if (tree >= a.cfg.n_trees) return;              // whole lane groups: no live lane of a group leaves here
@@ -82,7 +81,6 @@ __global__ void __launch_bounds__(128, 8) brue_kernel(BrueArgs a) {
     const b2_brue_tree& tr = a.tree;
     int32_t* path = tr.path + (int64_t)tree * H;
     double* path_reward = tr.path_reward + (int64_t)tree * H;
-    float* gs = scratch[(threadIdx.x >> 4) % (128 / 16)];
 
     Pcg64 rng;
     rng.load(a.rng + (int64_t)tree * B2_PCG64_STATE_WORDS);
@@ -101,7 +99,7 @@ __global__ void __launch_bounds__(128, 8) brue_kernel(BrueArgs a) {
         for (int h = 0; h < H; ++h) {                // rollout (:24-33)
             const int action = (int)rng.integers((uint32_t)a.cfg.n_actions);
             bool term, trunc;
-            const double r = env.step(a.cfg.mdp, action, li, gmask, gs, term, trunc);
+            const double r = env.step(a.cfg.mdp, action, li, gmask, term, trunc);
             if (writer) {                            // update's forward pass (:39-44)
                 // DecisionNode.get_child: the chance child of this action, appended to the list on the first visit
                 int c = tr.first_child[nb + node], last = -1;

@@ -42,7 +42,7 @@ struct FiniteEnv {
     __device__ __forceinline__ static int nth(int mask, int n) { return n; }
     // position of `action` among the available actions in the env's order, or -1
     __device__ __forceinline__ static int rank_of(int mask, int action) { return (action >= 0 && (mask >> action) & 1) ? action : -1; }
-    __device__ __forceinline__ double step(const b2_finite_mdp& m, int action, int li, unsigned gmask, float* gs,
+    __device__ __forceinline__ double step(const b2_finite_mdp& m, int action, int li, unsigned gmask,
                                            bool& term, bool& trunc) {
         const double r = m.reward[(int64_t)s * m.n_actions + action];
         term = m.terminal[s] != 0;        // finite_mdp's MDP.step: done = terminal[state BEFORE the transition]
@@ -75,9 +75,9 @@ struct HighwayEnv {
         }
         return -1;
     }
-    __device__ __forceinline__ double step(const b2_finite_mdp& m, int action, int li, unsigned gmask, float* gs,
+    __device__ __forceinline__ double step(const b2_finite_mdp& m, int action, int li, unsigned gmask,
                                            bool& term, bool& trunc) {
-        return (double)hw::step(L, li, t, si, action, term, trunc, gmask, gs);
+        return (double)hw::step(L, li, t, si, action, term, trunc, gmask);
     }
 };
 

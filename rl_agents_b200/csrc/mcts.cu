@@ -33,7 +33,6 @@ struct MctsArgs {
 template <class Env>
 __global__ void __launch_bounds__(128, B2_MCTS_MIN_BLOCKS) mcts_kernel(MctsArgs a) {
     constexpr int G = Env::GROUP;
-    __shared__ float scratch[G == 16 ? 128 / 16 : 1][hw::SCRATCH_FLOATS];
     const int gtid = blockIdx.x * 128 + threadIdx.x;
     const int tree_raw = gtid / G, li = gtid % G;
     const bool live = tree_raw < a.cfg.n_trees;
@@ -135,7 +134,7 @@ __global__ void __launch_bounds__(128, B2_MCTS_MIN_BLOCKS) mcts_kernel(MctsArgs 
             }
             bool term, trunc;
             Env next = env;
-            const double r = next.step(a.cfg.mdp, action, li, gmask, scratch[(threadIdx.x >> 4) % (128 / 16)], term, trunc);
+            const double r = next.step(a.cfg.mdp, action, li, gmask, term, trunc);
             if (active) {
                 env = next;
                 ++env_steps;

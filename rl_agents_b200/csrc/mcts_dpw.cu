@@ -59,7 +59,7 @@ struct DpwFinite {
     __device__ __forceinline__ int obs_key(const b2_mcts_dpw_config& c) const { return c.obs_keys[s]; }
     // -> the reward; bad_row >= 0: the row Generator.choice rejects (the state is left as it was)
     __device__ __forceinline__ double step(const b2_mcts_dpw_config& c, int action, Pcg64& env_rng, int li,
-                                           unsigned gmask, float* gs, bool& term, bool& trunc, int& bad_row) {
+                                           unsigned gmask, bool& term, bool& trunc, int& bad_row) {
         const b2_finite_mdp_sampled& m = c.mdp;
         const int64_t row = (int64_t)s * m.n_actions + action;
         if (c.env_draws && !m.row_ok[row]) { bad_row = (int)row; return 0.0; }
@@ -84,8 +84,8 @@ struct DpwHighway {
     // deterministic, so a chance node has one child either way.
     __device__ __forceinline__ int obs_key(const b2_mcts_dpw_config& c) const { return e.t; }
     __device__ __forceinline__ double step(const b2_mcts_dpw_config& c, int action, Pcg64& env_rng, int li,
-                                           unsigned gmask, float* gs, bool& term, bool& trunc, int& bad_row) {
-        return e.step(b2_finite_mdp{}, action, li, gmask, gs, term, trunc);
+                                           unsigned gmask, bool& term, bool& trunc, int& bad_row) {
+        return e.step(b2_finite_mdp{}, action, li, gmask, term, trunc);
     }
 };
 
@@ -103,14 +103,12 @@ __device__ __forceinline__ void new_node(const b2_mcts_dpw_tree& tr, int64_t nb,
 template <class Env>
 __global__ void __launch_bounds__(128, Env::GROUP == 16 ? 4 : 8) mcts_dpw_kernel(DpwArgs a) {
     constexpr int G = Env::GROUP;
-    __shared__ float scratch[G == 16 ? 128 / 16 : 1][G == 16 ? hw::SCRATCH_FLOATS : 1];
     const int gtid = blockIdx.x * 128 + threadIdx.x;
     const int tree = gtid / G, li = gtid % G;
     if (tree >= a.cfg.n_trees) return;              // whole lane groups: no live lane of a group leaves here
     const bool writer = li == 0;
     const int lane = threadIdx.x & 31;
     const unsigned gmask = G == 1 ? (1u << lane) : (0xFFFFu << (lane & 16));
-    float* gs = scratch[G == 16 ? (threadIdx.x >> 4) % (128 / 16) : 0];
     const b2_mcts_dpw_config& c = a.cfg;
     const b2_mcts_dpw_tree& tr = a.tree;
     const int A = c.n_actions, H = c.horizon;
@@ -170,7 +168,7 @@ __global__ void __launch_bounds__(128, Env::GROUP == 16 ? 4 : 8) mcts_dpw_kernel
                 }
                 action = tr.key[nb + chance];
             }
-            const double r = env.step(c, action, env_rng, li, gmask, gs, term, trunc, bad_row);
+            const double r = env.step(c, action, env_rng, li, gmask, term, trunc, bad_row);
             if (bad_row >= 0) { error = ERR_BAD_ROW; break; }
             ++steps;
             // ChanceNode.get_child (:171-182)
@@ -212,7 +210,7 @@ __global__ void __launch_bounds__(128, Env::GROUP == 16 ? 4 : 8) mcts_dpw_kernel
                 for (int i = 0; i < n; ++i) idx += cdf[i] <= u ? 1 : 0;   // searchsorted(side='right')
                 idx = min(idx, n - 1);
                 const int action = c.rollout_policy != 1 ? Env::nth(pm, idx) : idx;
-                const double r = env.step(c, action, env_rng, li, gmask, gs, term, trunc, bad_row);
+                const double r = env.step(c, action, env_rng, li, gmask, term, trunc, bad_row);
                 if (bad_row >= 0) { error = ERR_BAD_ROW; break; }
                 ++steps;
                 total = total + c.gamma_pow[h] * r;

@@ -22,7 +22,6 @@ namespace mwave {
 
 constexpr int THREADS = 256;
 constexpr int WARPS = THREADS / 32;
-constexpr int GROUPS = THREADS / 16;
 constexpr int MAX_WIDTH = 1024;
 constexpr int MAX_A = 8;
 constexpr int MAX_H = 64;
@@ -298,7 +297,6 @@ __device__ __forceinline__ void backup(const Args& a, int j, int reached, double
 __global__ void __launch_bounds__(THREADS, 1) mcts_wave_kernel(Args a) {
     extern __shared__ long long score_table[];
     __shared__ SelShared sh;
-    __shared__ float hw_scratch[GROUPS][hw::SCRATCH_FLOATS];
     const int tid = threadIdx.x, lane = tid & 31, li = tid & 15;
     const unsigned n_ctas = gridDim.x;
     Control* ctl = a.ctl;
@@ -346,12 +344,11 @@ __global__ void __launch_bounds__(THREADS, 1) mcts_wave_kernel(Args a) {
                 double total = 0.0;
                 bool terminal = false;
                 int reached = 0, steps = 0;
-                float* gs = hw_scratch[tid >> 4];
                 for (int h = 0; h < depth; ++h) {                               // mcts.py:141-149
                     const int node = __ldcg(a.paths + (int64_t)jj * H + h);
                     const int action = __ldcg(tr.meta + node) & 0xff;
                     bool term, trunc;
-                    const float r = hw::step(L, li, t, si, action, term, trunc, gmask, gs);
+                    const float r = hw::step(L, li, t, si, action, term, trunc, gmask);
                     ++steps;
                     total += a.cfg.gamma_pow[h] * (double)r;
                     reached = h + 1;
@@ -378,7 +375,7 @@ __global__ void __launch_bounds__(THREADS, 1) mcts_wave_kernel(Args a) {
                         const int mask = hw::avail_mask(ego_y, si);
                         const int action = hw::nth_action(mask, wave_random(a.cfg.seed, e, h, 1, __popc(mask)));
                         bool term, trunc;
-                        const float r = hw::step(L, li, t, si, action, term, trunc, gmask, gs);
+                        const float r = hw::step(L, li, t, si, action, term, trunc, gmask);
                         ++steps;
                         total += a.cfg.gamma_pow[h] * (double)r;
                         if (term || trunc) break;

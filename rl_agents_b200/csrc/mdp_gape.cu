@@ -122,7 +122,6 @@ __device__ __forceinline__ void new_node(const b2_mdp_gape_tree& tr, int64_t nb,
 template <class Env>
 __global__ void __launch_bounds__(128, 8) mdp_gape_kernel(GapeArgs a) {
     constexpr int G = Env::GROUP;
-    __shared__ float scratch[G == 16 ? 128 / 16 : 1][hw::SCRATCH_FLOATS];
     const int gtid = blockIdx.x * 128 + threadIdx.x;
     const int tree = gtid / G, li = gtid % G;
     if (tree >= a.cfg.n_trees) return;              // whole lane groups: no live lane of a group leaves here
@@ -133,7 +132,6 @@ __global__ void __launch_bounds__(128, 8) mdp_gape_kernel(GapeArgs a) {
     const int64_t nb = (int64_t)tree * a.cfg.node_capacity;
     const b2_mdp_gape_tree& tr = a.tree;
     const double gamma = a.cfg.gamma;
-    float* gs = scratch[(threadIdx.x >> 4) % (128 / 16)];
 
     Pcg64 rng;
     rng.load(a.rng + (int64_t)tree * B2_PCG64_STATE_WORDS);
@@ -199,7 +197,7 @@ __global__ void __launch_bounds__(128, 8) mdp_gape_kernel(GapeArgs a) {
                 if ((tr.meta[nb + fc + i] & 0xff) == action) { chance = fc + i; break; }
             action = tr.meta[nb + chance] & 0xff;
             bool term, trunc;
-            const double r = env.step(a.cfg.mdp, action, li, gmask, gs, term, trunc);          // :82
+            const double r = env.step(a.cfg.mdp, action, li, gmask, term, trunc);          // :82
             // ChanceNode.get_child (:272-286): placeholders on the first visit, the observation takes placeholder 0
             int child = tr.first_child[nb + chance];
             if (child < 0) {

@@ -27,7 +27,6 @@ struct OlopArgs {
 template <class Env>
 __global__ void __launch_bounds__(128, 8) olop_kernel(OlopArgs a) {
     constexpr int G = Env::GROUP;
-    __shared__ float scratch[G == 16 ? 128 / 16 : 1][hw::SCRATCH_FLOATS];
     const int gtid = blockIdx.x * 128 + threadIdx.x;
     const int tree_raw = gtid / G, li = gtid % G;
     const bool live = tree_raw < a.cfg.n_trees;
@@ -98,8 +97,7 @@ __global__ void __launch_bounds__(128, 8) olop_kernel(OlopArgs a) {
                 action = tr.meta[nb + child] & 0xff;
             }
             bool term, trunc;
-            const double r = env.step(a.cfg.mdp, action, li, gmask, scratch[(threadIdx.x >> 4) % (128 / 16)], term,
-                                      trunc);     // olop.py:87
+            const double r = env.step(a.cfg.mdp, action, li, gmask, term, trunc);     // olop.py:87
             if (live && !error) {
                 node = child;
                 // update (olop.py:132-142)

@@ -264,7 +264,6 @@ constexpr int HW_THREADS = 96;
 __global__ void __launch_bounds__(HW_THREADS) opd_highway_kernel(OpdArgs a) {
     extern __shared__ double smem_d[];
     __shared__ Shared sh;
-    __shared__ float hw_scratch[HW_THREADS / 16][hw::SCRATCH_FLOATS];
     const int tree_id = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int grp = tid >> 4, li = tid & 15;
     const int64_t nb = (int64_t)tree_id * a.cfg.node_capacity;
@@ -299,7 +298,7 @@ __global__ void __launch_bounds__(HW_THREADS) opd_highway_kernel(OpdArgs a) {
         const int n = __popc(mask);
         const int action = grp < n ? hw::nth_action(mask, grp) : hw::A_IDLE;
         bool term, trunc;
-        const float r = hw::step(L, li, t, si, action, term, trunc, 0xffffffffu, hw_scratch[grp]);
+        const float r = hw::step(L, li, t, si, action, term, trunc, 0xffffffffu);
         if (grp < n) {
             hw::store_state(states + (int64_t)(n_nodes + grp) * hw::WORDS, li, L, t, si);
             if (li == 0) {
@@ -346,10 +345,9 @@ struct MultiShared {
 __global__ void __launch_bounds__(MT_THREADS, B2_MT_MIN_BLOCKS) opd_highway_multi_kernel(OpdArgs a) {
     extern __shared__ double smem_d[];
     __shared__ MultiShared ms;
-    __shared__ float hw_scratch[MT_GROUPS][hw::SCRATCH_FLOATS];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, li = tid & 15;
     int grp = tid >> 4;
-    asm volatile("" : "+r"(grp));   // keep in a register (else re-derived from SR_TID.X at every scratch access)
+    asm volatile("" : "+r"(grp));   // keep in a register (else re-derived from SR_TID.X)
     const int tree0 = blockIdx.x * MT_TREES;
     const int n_local = min(MT_TREES, a.cfg.n_trees - tree0);
     // the warp's own tree
@@ -416,7 +414,7 @@ __global__ void __launch_bounds__(MT_THREADS, B2_MT_MIN_BLOCKS) opd_highway_mult
             hw::load_state(states + (int64_t)sh.leaf * hw::WORDS, li, L, t, si);
             const int action = real ? hw::nth_action(ms.mask[tr], k) : hw::A_IDLE;
             bool term, trunc;
-            const float r = hw::step(L, li, t, si, action, term, trunc, 0xffffffffu, hw_scratch[grp]);
+            const float r = hw::step(L, li, t, si, action, term, trunc, 0xffffffffu);
             if (real) {
                 hw::store_state(states + (int64_t)(ms.n_nodes[tr] + k) * hw::WORDS, li, L, t, si);
                 if (li == 0) {
@@ -549,7 +547,6 @@ __device__ __forceinline__ void flow_commit(const OpdArgs& a, FlowShared& fs, in
 __global__ void __launch_bounds__(MT_THREADS, B2_MT_MIN_BLOCKS) opd_highway_flow_kernel(OpdArgs a) {
     extern __shared__ double smem_d[];
     __shared__ FlowShared fs;
-    __shared__ float hw_scratch[MT_GROUPS][hw::SCRATCH_FLOATS];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, li = tid & 15, half = (tid >> 4) & 1;
     int grp = tid >> 4;
     asm volatile("" : "+r"(grp));
@@ -602,7 +599,7 @@ __global__ void __launch_bounds__(MT_THREADS, B2_MT_MIN_BLOCKS) opd_highway_flow
             hw::load_state(states + (int64_t)fs.sh[tr].leaf * hw::WORDS, li, L, t, si);
             const int action = real ? hw::nth_action(fs.mask[tr], k) : hw::A_IDLE;
             bool term, trunc;
-            const float r = hw::step(L, li, t, si, action, term, trunc, 0xffffffffu, hw_scratch[grp]);
+            const float r = hw::step(L, li, t, si, action, term, trunc, 0xffffffffu);
             if (real) {
                 hw::store_state(states + (int64_t)(fs.c0[tr] + k) * hw::WORDS, li, L, t, si);
                 if (li == 0) {
@@ -656,14 +653,12 @@ constexpr int WT_WARPS = 4;
 __global__ void __launch_bounds__(WT_WARPS * 32, B2_WT_MIN_BLOCKS) opd_highway_warp_kernel(OpdArgs a) {
     extern __shared__ double smem_d[];
     __shared__ Shared shs[WT_WARPS];
-    __shared__ float hw_scratch[WT_WARPS * 2][hw::SCRATCH_FLOATS];
     const int tid = threadIdx.x, lane = tid & 31, li = tid & 15, half = (tid >> 4) & 1;
     int warp = tid >> 5;
     asm volatile("" : "+r"(warp));
     const int tree_id = blockIdx.x * WT_WARPS + warp;
     if (tree_id >= a.cfg.n_trees) return;        // whole warp; nothing below synchronises across warps
     Shared& sh = shs[warp];
-    float* gs = hw_scratch[warp * 2 + half];
     const int64_t nb = (int64_t)tree_id * a.cfg.node_capacity;
     char* ws = a.workspace + (int64_t)tree_id * a.lay.ws_bytes_per_tree;
     Tournament T;
@@ -695,7 +690,7 @@ __global__ void __launch_bounds__(WT_WARPS * 32, B2_WT_MIN_BLOCKS) opd_highway_w
             hw::Lane L = P;
             int t = pt, si = psi;
             bool term, trunc;
-            const float r = hw::step(L, li, t, si, action, term, trunc, 0xffffffffu, gs);
+            const float r = hw::step(L, li, t, si, action, term, trunc, 0xffffffffu);
             if (real) {
                 hw::store_state(states + (int64_t)(n_nodes + k) * hw::WORDS, li, L, t, si);
                 if (li == 0) {
@@ -721,7 +716,6 @@ __global__ void __launch_bounds__(WT_WARPS * 32, B2_WT_MIN_BLOCKS) opd_highway_w
 // ---------------------------------------------------------------------------
 __global__ void __launch_bounds__(128) highway_step_kernel(int32_t* states, const int32_t* actions, float* reward,
                                                            int32_t* flags, int32_t* avail, int n_envs) {
-    __shared__ float hw_scratch[128 / 16][hw::SCRATCH_FLOATS];
     const int g = (blockIdx.x * 128 + threadIdx.x) >> 4, li = threadIdx.x & 15;
     const bool live = g < n_envs;
     const int e = live ? g : n_envs - 1;
@@ -729,7 +723,7 @@ __global__ void __launch_bounds__(128) highway_step_kernel(int32_t* states, cons
     int t, si;
     hw::load_state(states + (int64_t)e * hw::WORDS, li, L, t, si);
     bool term, trunc;
-    const float r = hw::step(L, li, t, si, actions[e], term, trunc, 0xffffffffu, hw_scratch[threadIdx.x >> 4]);
+    const float r = hw::step(L, li, t, si, actions[e], term, trunc, 0xffffffffu);
     const float ego_y = __shfl_sync(0xffffffffu, L.y, 0, 16);
     if (live) {
         hw::store_state(states + (int64_t)e * hw::WORDS, li, L, t, si);

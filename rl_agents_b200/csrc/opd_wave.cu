@@ -31,7 +31,6 @@ namespace wave {
 #endif
 constexpr int THREADS = B2_WAVE_THREADS;
 constexpr int WARPS = THREADS / 32;
-constexpr int GROUPS = THREADS / 16;
 constexpr int STAGE_CAP = 24576;            // fp64 keys staged in shared memory per tile (192 KB)
 constexpr int MAX_BRANCH = 8;
 
@@ -713,7 +712,6 @@ __device__ void finish_tree(const Args& a, long long tp) {
 __global__ void __launch_bounds__(THREADS, 1) opd_wave_kernel(Args a) {
     extern __shared__ unsigned long long skeys[];
     __shared__ SelShared sh;
-    __shared__ float hw_scratch[GROUPS][hw::SCRATCH_FLOATS];
     __shared__ int s_nodes, s_expanded, s_staged;
     const int tid = threadIdx.x, lane = tid & 31, li = tid & 15;
     const unsigned n_ctas = gridDim.x;
@@ -806,7 +804,7 @@ __global__ void __launch_bounds__(THREADS, 1) opd_wave_kernel(Args a) {
                 int t, si;
                 load_state_cg(tr.state + ((int64_t)leaf * Mx + m) * hw::WORDS, li, L, t, si);
                 bool term, trunc;
-                const float r = hw::step(L, li, t, si, action, term, trunc, 0xffffffffu, hw_scratch[tid >> 4]);
+                const float r = hw::step(L, li, t, si, action, term, trunc, 0xffffffffu);
                 const float ego_y = __shfl_sync(0xffffffffu, L.y, 0, 16);
                 if (real) {
                     const int c = base + w;
@@ -919,7 +917,6 @@ __global__ void __launch_bounds__(THREADS, 1) opd_spec_kernel(Args a) {
     extern __shared__ unsigned long long skeys[];
     __shared__ SelShared sh;
     __shared__ SpecShared sp;
-    __shared__ float hw_scratch[GROUPS][hw::SCRATCH_FLOATS];
     __shared__ int s_nodes, s_expanded, s_slots;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, li = tid & 15;
     const unsigned n_ctas = gridDim.x;
@@ -1035,7 +1032,7 @@ __global__ void __launch_bounds__(THREADS, 1) opd_spec_kernel(Args a) {
                     hw::Lane L;
                     int t, si;
                     load_state_cg(src, li, L, t, si);
-                    r = hw::step(L, li, t, si, action, term, trunc, 0xffffffffu, hw_scratch[tid >> 4]);
+                    r = hw::step(L, li, t, si, action, term, trunc, 0xffffffffu);
                     const float ego_y = __shfl_sync(0xffffffffu, L.y, 0, 16);
                     avail = hw::avail_mask(ego_y, si);
                     if (real) hw::store_state(dst, li, L, t, si);

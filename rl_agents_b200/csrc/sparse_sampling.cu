@@ -82,14 +82,14 @@ __device__ __forceinline__ void put(const b2_sparse_sampling_tree& tr, int64_t n
 
 struct SFiniteEnv {
     static constexpr int GROUP = 1;
-    __device__ __forceinline__ int root(const SsArgs& a, int tree, int li, unsigned gmask, float* gs) {
+    __device__ __forceinline__ int root(const SsArgs& a, int tree, int li, unsigned gmask) {
         return a.root_states[tree];
     }
     __device__ __forceinline__ int n_choices(const SsArgs& a, int state) const { return a.cfg.n_actions; }
     __device__ __forceinline__ int action(int state, int idx) const { return idx; }   // range(action_space.n), :40-43
     // estimateQ's sampling loop (:76-84) for `action` in frame d: C samples, the distinct next states in first-visit
     // order with their counts, each a new DecisionNode.  Returns the reward; sets err / bad_row on a rejected row.
-    __device__ __forceinline__ double expand(const SsArgs& a, int tree, int li, unsigned gmask, float* gs, int d,
+    __device__ __forceinline__ double expand(const SsArgs& a, int tree, int li, unsigned gmask, int d,
                                              int state, int action, int chance, Pcg64& rng, int& n_nodes, int& nk,
                                              int& err, int& bad_row) {
         const b2_finite_mdp_sampled& m = a.cfg.mdp;
@@ -137,7 +137,7 @@ struct SHighwayEnv {
     __device__ __forceinline__ int32_t* words(const SsArgs& a, int tree, int d) const {
         return a.st.hw + ((int64_t)tree * (a.cfg.horizon + 1) + d) * hw::WORDS;
     }
-    __device__ __forceinline__ int root(const SsArgs& a, int tree, int li, unsigned gmask, float* gs) {
+    __device__ __forceinline__ int root(const SsArgs& a, int tree, int li, unsigned gmask) {
         hw::Lane L;
         int t, si;
         hw::load_state(a.root_states + (int64_t)tree * hw::WORDS, li, L, t, si);
@@ -147,7 +147,7 @@ struct SHighwayEnv {
     }
     __device__ __forceinline__ int n_choices(const SsArgs& a, int mask) const { return __popc(mask); }
     __device__ __forceinline__ int action(int mask, int idx) const { return hw::nth_action(mask, idx); }
-    __device__ __forceinline__ double expand(const SsArgs& a, int tree, int li, unsigned gmask, float* gs, int d,
+    __device__ __forceinline__ double expand(const SsArgs& a, int tree, int li, unsigned gmask, int d,
                                              int mask, int action, int chance, Pcg64& rng, int& n_nodes, int& nk,
                                              int& err, int& bad_row) {
         const Stack& st = a.st;
@@ -157,7 +157,7 @@ struct SHighwayEnv {
         int t, si;
         hw::load_state(words(a, tree, d), li, L, t, si);
         bool term, trunc;                                           // `done` is ignored (:81)
-        const float r = hw::step(L, li, t, si, action, term, trunc, gmask, gs);
+        const float r = hw::step(L, li, t, si, action, term, trunc, gmask);
         int child_mask = 0;
         if (d + 1 < a.cfg.horizon) {
             hw::store_state(words(a, tree, d + 1), li, L, t, si);
@@ -182,14 +182,12 @@ struct SHighwayEnv {
 template <class Env>
 __global__ void __launch_bounds__(128, Env::GROUP == 16 ? 4 : 8) sparse_sampling_kernel(SsArgs a) {
     constexpr int G = Env::GROUP;
-    __shared__ float scratch[G == 16 ? 128 / 16 : 1][G == 16 ? hw::SCRATCH_FLOATS : 1];
     const int gtid = blockIdx.x * 128 + threadIdx.x;
     const int tree = gtid / G, li = gtid % G;
     if (tree >= a.cfg.n_trees) return;              // whole lane groups: no live lane of a group leaves here
     const bool writer = li == 0;
     const int lane = threadIdx.x & 31;
     const unsigned gmask = G == 1 ? (1u << lane) : (0xFFFFu << (lane & 16));
-    float* gs = scratch[G == 16 ? (threadIdx.x >> 4) % (128 / 16) : 0];
     const int H = a.cfg.horizon, C = a.cfg.C, n = a.cfg.n_trees, A = a.cfg.n_actions;
     const Stack& st = a.st;
     const b2_sparse_sampling_tree& tr = a.tree;
@@ -206,7 +204,7 @@ __global__ void __launch_bounds__(128, Env::GROUP == 16 ? 4 : 8) sparse_sampling
     }
     // Every lane of a group keeps the same counters and writes the same frame words; only lane 0 writes the dump.
     int n_nodes = 1, n_chance = 0, samples = 0, error = 0, bad_row = -1;
-    const int root_choice = env.root(a, tree, li, gmask, gs);
+    const int root_choice = env.root(a, tree, li, gmask);
     st.state[tree] = root_choice;
     st.node[tree] = 0;
     st.act[tree] = 0;
@@ -222,7 +220,7 @@ __global__ void __launch_bounds__(128, Env::GROUP == 16 ? 4 : 8) sparse_sampling
             ++n_chance;
             if (rec && writer) put(tr, nb, c, st.node[f], KIND_CHANCE, action, d);
             int nk = 0;
-            const double r = env.expand(a, tree, li, gmask, gs, d, s, action, c, rng, n_nodes, nk, error, bad_row);
+            const double r = env.expand(a, tree, li, gmask, d, s, action, c, rng, n_nodes, nk, error, bad_row);
             samples += error ? 1 : C;
             if (error) break;
             st.chance[f] = c;
