@@ -83,6 +83,15 @@ int b2_intersection_step(int32_t* states, const int32_t* actions, float* reward,
  * mantissa, both signs and exponents -60..60, and writes the number of differing results (must be 0). */
 int b2_selftest_const_division(unsigned long long* mismatches_dev, void* stream);
 
+/* Self-test (tests/test_gpu_highway_step_paths.py): the HighwayLite step in the per-group mode of the
+ * one-tree-per-group planners -- scene s on its own 16-lane group (HighwayEnv::step, that group's mask),
+ * n_steps[s] <= max_steps decisions.  actions [n_scenes, max_steps]; every intermediate state to
+ * trace [n_scenes, max_steps, 136]; reward [n_scenes, max_steps]; flags [n_scenes, max_steps] = bit0 terminated,
+ * bit1 truncated, available-action mask of the new state << 2.  Entries past n_steps[s] are left as they were. */
+int b2_selftest_highway_step_groups(const int32_t* states, const int32_t* actions, const int32_t* n_steps,
+                                    int32_t* trace, float* reward, int32_t* flags, int32_t n_scenes,
+                                    int32_t max_steps, void* stream);
+
 /* ------------------------------------------------------------------------
  * Value iteration -- rl_agents/agents/dynamic_programming/value_iteration.py
  * ---------------------------------------------------------------------- */

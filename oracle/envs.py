@@ -359,9 +359,17 @@ def highway_available_actions(state):
     return actions
 
 
-def highway_step(state, action):
+def highway_step(state, action, on_substep=None):
     """One decision step (15 sub-steps) in place; returns (reward f32,
-    terminated, truncated)."""
+    terminated, truncated).
+
+    `on_substep`, when given, is called once per sub-step, after the lane
+    decisions and before the integration, with keyword arguments (arrays over
+    the 16 slots, read-only): sub, x, y, v, present, crashed (as of the
+    sub-step start), cur, tgt (target lanes at the sub-step start), new_tgt,
+    decide (MOBIL deciders), abort (abort rule fired), wrapped (heading error
+    wrapped by 2*pi) and clamped (|v| > MAX_SPEED).  It observes only: the
+    step computes the same values with or without it."""
     s = state
     n = V_SLOTS
     idx = np.arange(n)
@@ -381,7 +389,7 @@ def highway_step(state, action):
     elif action == A_RIGHT:
         s.tgt_lane[0] = min(int(s.tgt_lane[0]) + 1, N_LANES - 1)
 
-    for _ in range(SUBSTEPS):
+    for sub in range(SUBSTEPS):
         x, y, h, v = s.x, s.y, s.h, s.v
         cur = np.clip(np.rint(y / LANE_W), 0, N_LANES - 1).astype(np.int32)
         cur_y = cur.astype(f32) * LANE_W
@@ -426,6 +434,10 @@ def highway_step(state, action):
         u = np.minimum(np.maximum(u, -QUARTER_PI_SIN), QUARTER_PI_SIN)
         heading_ref = asin_p(u)
         dh = heading_ref - h
+        if on_substep is not None:
+            wrapped = (dh > PI) | (np.where(dh > PI, dh - TWO_PI, dh) < -PI)
+            on_substep(sub=sub, x=x, y=y, v=v, present=present, crashed=crashed, cur=cur, tgt=s.tgt_lane,
+                       new_tgt=tgt, decide=decide, abort=abort, wrapped=wrapped, clamped=np.abs(v) > MAX_SPEED)
         dh = np.where(dh > PI, dh - TWO_PI, dh)
         dh = np.where(dh < -PI, dh + TWO_PI, dh)
         dh = np.where(np.abs(dh) < HEADING_DEADBAND, f32(0.0), dh).astype(f32)

@@ -203,6 +203,7 @@ EXPORTS = {
     "b2_device_info": (c_int, [ctypes.POINTER(c_int)] * 3 + [ctypes.c_char_p, c_int]),
     "b2_intersection_step": (c_int, [c_void_p] * 5 + [c_int32, c_void_p]),
     "b2_selftest_const_division": (c_int, [c_void_p, c_void_p]),
+    "b2_selftest_highway_step_groups": (c_int, [c_void_p] * 6 + [c_int32, c_int32, c_void_p]),
     "b2_highway_step": (c_int, [c_void_p] * 5 + [c_int32, c_void_p]),
     "b2_highway_ttc_vi": (c_int, [c_void_p, c_int32, c_double, c_int32, c_double, c_double] + [c_void_p] * 5),
     "b2_vi_sweep": (c_int, [ctypes.POINTER(VIProblem)] + [c_void_p] * 5 + [c_int32, c_void_p]),

@@ -20,6 +20,7 @@
 //     node exactly (max and integer sums are order independent).
 #include "common.cuh"
 #include "highway_lite.cuh"
+#include "lane_env.cuh"
 
 namespace b2 {
 
@@ -778,6 +779,33 @@ __global__ void const_division_selftest_kernel(unsigned long long* mismatches) {
     if (bad) atomicAdd(mismatches, bad);
 }
 
+// Test entry of hw::step in the per-group mode of the one-tree-per-group planners (mcts.cu, olop.cu, ...): scene s on
+// its own 16-lane group through HighwayEnv::step with that group's gmask, n_steps[s] decisions each, so the two groups
+// of a warp step different numbers of times.  Decision k of scene s reads actions[s * max_steps + k] and writes the new
+// state to trace[(s * max_steps + k) * 136 ..] and reward / flags (bit0 terminated, bit1 truncated, avail mask << 2)
+// to out[s * max_steps + k].
+__global__ void __launch_bounds__(64) highway_step_groups_kernel(const int32_t* states, const int32_t* actions,
+                                                                const int32_t* n_steps, int32_t* trace, float* reward,
+                                                                int32_t* flags, int n_scenes, int max_steps) {
+    const int lane = threadIdx.x & 31, li = lane & 15;
+    const int s = (blockIdx.x * 64 + threadIdx.x) >> 4;
+    if (s >= n_scenes) return;       // a whole group leaves: the other group of the warp works alone
+    const unsigned gmask = 0xFFFFu << (lane & 16);
+    HighwayEnv env;
+    env.load_root(states, s, li);
+    for (int k = 0; k < n_steps[s]; ++k) {
+        const int64_t o = (int64_t)s * max_steps + k;
+        bool term, trunc;
+        const float r = (float)env.step(b2_finite_mdp{}, actions[o], li, gmask, term, trunc);
+        const int avail = env.avail(hw::A_SLOWER + 1, gmask);
+        hw::store_state(trace + o * hw::WORDS, li, env.L, env.t, env.si);
+        if (li == 0) {
+            reward[o] = r;
+            flags[o] = (term ? 1 : 0) | (trunc ? 2 : 0) | (avail << 2);
+        }
+    }
+}
+
 static int make_layout(const b2_opd_config* cfg, LevelLayout* lay, int smem_budget_doubles) {
     int n = cfg->node_capacity, l = 0;
     lay->n_levels = 0;
@@ -881,6 +909,17 @@ extern "C" int b2_selftest_const_division(unsigned long long* mismatches_dev, vo
     B2_REQUIRE(mismatches_dev, "null pointer");
     B2_CUDA_CHECK(cudaMemsetAsync(mismatches_dev, 0, 8, (cudaStream_t)stream));
     const_division_selftest_kernel<<<(1u << 23) / 256, 256, 0, (cudaStream_t)stream>>>(mismatches_dev);
+    B2_CUDA_CHECK(cudaGetLastError());
+    return B2_OK;
+}
+
+extern "C" int b2_selftest_highway_step_groups(const int32_t* states, const int32_t* actions, const int32_t* n_steps,
+                                               int32_t* trace, float* reward, int32_t* flags, int32_t n_scenes,
+                                               int32_t max_steps, void* stream) {
+    B2_REQUIRE(states && actions && n_steps && trace && reward && flags && n_scenes > 0 && max_steps > 0,
+               "null pointer / empty batch");
+    highway_step_groups_kernel<<<(n_scenes + 3) / 4, 64, 0, (cudaStream_t)stream>>>(states, actions, n_steps, trace,
+                                                                                    reward, flags, n_scenes, max_steps);
     B2_CUDA_CHECK(cudaGetLastError());
     return B2_OK;
 }
