@@ -642,6 +642,23 @@ int b2_sparse_sampling_plan(const b2_sparse_sampling_config* cfg, const int32_t*
                             const b2_sparse_sampling_tree* tree, void* workspace, uint64_t* rng, double* root_q,
                             int8_t* plan, int32_t* result, void* stream);
 
+/* Bytes of scratch b2_sparse_sampling_plan_levels needs, sized for the worst case in which every decision node has
+ * all n_actions actions: per-node ints and fp64 values for every level and, on HighwayLite, two levels of
+ * n_actions^(horizon - 1) scenes.  0 for a config that call refuses. */
+int64_t b2_sparse_sampling_levels_workspace_bytes(const b2_sparse_sampling_config* cfg);
+
+/* The same decision as b2_sparse_sampling_plan -- every output bit for bit, the dump's creation order included -- for
+ * ONE tree on a deterministic model (HighwayLite, or a finite MDP with mdp.n_next == 1), searched by the whole GPU
+ * level by level in one cooperative launch: level d's chance nodes are numbered by a prefix sum of its available-
+ * action counts and stepped in parallel, values are backed up level by level, and the planner's stream is skipped by
+ * C halves per chance node in closed form.  Refused (B2_ERR_INVALID): n_trees != 1, n_next != 1, horizon < 1,
+ * C < 1, null pointers, and a worst-case tree that does not fit int32 node ids.  mdp.cdf and mdp.row_ok are not
+ * read: a one-entry row always samples its one next state.  A dump capacity below the node count sets error 1; the
+ * other outputs are then unspecified. */
+int b2_sparse_sampling_plan_levels(const b2_sparse_sampling_config* cfg, const int32_t* root_states,
+                                   const b2_sparse_sampling_tree* tree, void* workspace, uint64_t* rng, double* root_q,
+                                   int8_t* plan, int32_t* result, void* stream);
+
 /* ------------------------------------------------------------------------
  * MCTS with double progressive widening -- rl_agents/agents/tree_search/mcts_dpw.py (MCTSDPW).  Finite MDPs in all
  * three modes (the env copy's `seed(np_random.randint(2**30))` once per run, then Generator.choice(p.size, p=p) per

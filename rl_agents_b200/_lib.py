@@ -250,6 +250,9 @@ EXPORTS = {
     "b2_sparse_sampling_workspace_bytes": (c_int64, [ctypes.POINTER(SparseSamplingConfig)]),
     "b2_sparse_sampling_plan": (c_int, [ctypes.POINTER(SparseSamplingConfig), c_void_p,
                                         ctypes.POINTER(SparseSamplingTree)] + [c_void_p] * 6),
+    "b2_sparse_sampling_levels_workspace_bytes": (c_int64, [ctypes.POINTER(SparseSamplingConfig)]),
+    "b2_sparse_sampling_plan_levels": (c_int, [ctypes.POINTER(SparseSamplingConfig), c_void_p,
+                                               ctypes.POINTER(SparseSamplingTree)] + [c_void_p] * 6),
     "b2_mcts_dpw_plan": (c_int, [ctypes.POINTER(MCTSDPWConfig), c_void_p, ctypes.POINTER(MCTSDPWTree), c_void_p,
                                  c_void_p, c_void_p, c_void_p]),
 }

@@ -39,6 +39,28 @@ int check_lane_env(int env_kind, int n_actions, const b2_finite_mdp& mdp);
 // Blocks of 128 threads for n_trees trees of `group` lanes each.
 inline int lane_grid(int n_trees, int group) { return (n_trees * group + 127) / 128; }
 
+// Grid-wide barrier of a cooperative launch (all CTAs co-resident), keyed on two control words of `ctl` that the launch
+// wrapper zeroes: the arrival count `bar_count` and the generation `bar_gen`.  Data written before it by any CTA is
+// visible to every CTA after it.
+template <class Control>
+__device__ __forceinline__ void grid_barrier(Control* ctl, unsigned n_ctas) {
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        volatile unsigned* gen_p = &ctl->bar_gen;
+        const unsigned gen = *gen_p;
+        __threadfence();
+        if (atomicAdd(&ctl->bar_count, 1u) == n_ctas - 1) {
+            ctl->bar_count = 0;
+            __threadfence();
+            atomicAdd(&ctl->bar_gen, 1u);
+        } else {
+            while (*gen_p == gen) {}
+        }
+        __threadfence();
+    }
+    __syncthreads();
+}
+
 __device__ __forceinline__ double warp_max_f64(double v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {

@@ -59,24 +59,6 @@ __device__ __forceinline__ int wave_random(unsigned long long seed, int episode,
     return (int)((unsigned)(splitmix64(key) >> 33) % (unsigned)n);    // 31-bit value: a 32-bit modulo gives the same result
 }
 
-__device__ __forceinline__ void grid_barrier(Control* ctl, unsigned n_ctas) {
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        volatile unsigned* gen_p = &ctl->bar_gen;
-        const unsigned gen = *gen_p;
-        __threadfence();
-        if (atomicAdd(&ctl->bar_count, 1u) == n_ctas - 1) {
-            ctl->bar_count = 0;
-            __threadfence();
-            atomicAdd(&ctl->bar_gen, 1u);
-        } else {
-            while (*gen_p == gen) {}
-        }
-        __threadfence();
-    }
-    __syncthreads();
-}
-
 // order-preserving image of a finite double as a signed 64-bit integer (+0 and -0 coincide)
 __device__ __forceinline__ long long score_key(double x) {
     const long long b = __double_as_longlong(x + 0.0);

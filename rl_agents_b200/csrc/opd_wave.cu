@@ -83,25 +83,7 @@ constexpr unsigned long long ABSENT = 0x000fffffffffffffull;   // image of -inf:
 __device__ __forceinline__ int ld_cg(const int32_t* p) { return __ldcg(p); }
 __device__ __forceinline__ double ld_cg(const double* p) { return __ldcg(p); }
 
-// grid-wide barrier (all CTAs are co-resident: cooperative launch).  Data written before it by any CTA is
-// read after it with ld.global.cg (L2) by the others.
-__device__ __forceinline__ void grid_barrier(Control* ctl, unsigned n_ctas) {
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        volatile unsigned* gen_p = &ctl->bar_gen;
-        const unsigned gen = *gen_p;
-        __threadfence();
-        if (atomicAdd(&ctl->bar_count, 1u) == n_ctas - 1) {
-            ctl->bar_count = 0;
-            __threadfence();
-            atomicAdd(&ctl->bar_gen, 1u);
-        } else {
-            while (*gen_p == gen) {}
-        }
-        __threadfence();
-    }
-    __syncthreads();
-}
+// Data written before a grid barrier (common.cuh) by any CTA is read after it with ld.global.cg (L2) by the others.
 
 __device__ __forceinline__ int block_sum(int v, int* red, int slot) {   // red: [2][WARPS]; slot alternates
     const int w = __reduce_add_sync(0xffffffffu, v);

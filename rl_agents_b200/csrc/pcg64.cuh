@@ -44,6 +44,31 @@ struct Pcg64 {
         uinteger = (uint32_t)(n >> 32);
         return (uint32_t)n;
     }
+    // The state after n calls of next32(), in O(log n): the buffered half first; then, for the m >= 1 halves left,
+    // floor((m - 1) / 2) LCG steps (pcg_advance_lcg_128: square-and-multiply of next64's affine map) and the last
+    // next64() as next32() runs it -- once when m is odd (its high half stays buffered), twice when m is even (the
+    // buffered word, `uinteger`, then holds that step's high half, as after the last of the n calls).
+    // CPU twin: tests/test_pcg64_skip.py::skip32.
+    __device__ __forceinline__ void skip32(uint64_t n) {
+        if (n == 0) return;
+        if (has_uint32) {
+            has_uint32 = 0;
+            if (--n == 0) return;
+        }
+        unsigned __int128 cur_mult = ((unsigned __int128)0x2360ED051FC65DA4ULL << 64) | 0x4385DF649FCCF645ULL;
+        unsigned __int128 cur_plus = inc, acc_mult = 1, acc_plus = 0;
+        for (uint64_t delta = (n - 1) >> 1; delta > 0; delta >>= 1) {
+            if (delta & 1) {
+                acc_mult *= cur_mult;
+                acc_plus = acc_plus * cur_mult + cur_plus;
+            }
+            cur_plus = (cur_mult + 1) * cur_plus;
+            cur_mult *= cur_mult;
+        }
+        state = acc_mult * state + acc_plus;
+        next32();
+        if (!(n & 1)) next32();
+    }
     __device__ __forceinline__ double random() { return (double)(next64() >> 11) * (1.0 / 9007199254740992.0); }
     // Generator.integers(0, n), 1 <= n < 2^32 (Lemire, buffered 32-bit halves)
     __device__ __forceinline__ uint32_t integers(uint32_t n) {

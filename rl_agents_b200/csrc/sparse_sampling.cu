@@ -27,12 +27,16 @@
 #include "highway_lite.cuh"
 #include "lane_env.cuh"
 #include "pcg64.cuh"
+#include "sparse_sampling.cuh"
 
 namespace b2 {
 namespace {
 
-constexpr int KIND_DECISION = 0, KIND_CHANCE = 1;
-constexpr int ERR_CAPACITY = 1, ERR_BAD_ROW = 2;
+using ss::KIND_DECISION;
+using ss::KIND_CHANCE;
+using ss::ERR_CAPACITY;
+using ss::ERR_BAD_ROW;
+using ss::put;
 
 // The search stack, tree index fastest (lanes at the same depth touch neighbouring words).  Frame d of tree t is
 // entry d * n + t; child j of frame d is entry (d * C + j) * n + t.
@@ -72,13 +76,6 @@ struct SsArgs {
     int8_t* plan;
     int32_t* result;
 };
-
-// DecisionNode / ChanceNode.__init__ (:32-36, :65-69): value 0, count 0
-__device__ __forceinline__ void put(const b2_sparse_sampling_tree& tr, int64_t nb, int id, int parent, int kind, int key,
-                                    int depth) {
-    tr.parent[nb + id] = parent; tr.kind[nb + id] = kind; tr.key[nb + id] = key; tr.depth[nb + id] = depth;
-    tr.count[nb + id] = 0; tr.value[nb + id] = 0.0;
-}
 
 struct SFiniteEnv {
     static constexpr int GROUP = 1;
@@ -271,20 +268,9 @@ __global__ void __launch_bounds__(128, Env::GROUP == 16 ? 4 : 8) sparse_sampling
 
     if (writer) {
         int action = -1;
-        if (!error) {                               // get_plan: root.selection_rule, random_argmax (:26-28, :53-56)
-            const int nc = env.n_choices(a, root_choice);
-            double m = root_q[env.action(root_choice, 0)];
-            int ties = 1;
-            for (int i = 1; i < nc; ++i) {
-                const double v = root_q[env.action(root_choice, i)];
-                if (v > m) { m = v; ties = 1; } else if (v == m) ++ties;
-            }
-            int pick = (int)rng.integers((uint32_t)ties);               // draws only for two or more ties
-            for (int i = 0; i < nc; ++i) {
-                const int act = env.action(root_choice, i);
-                if (root_q[act] == m && pick-- == 0) { action = act; break; }
-            }
-        }
+        if (!error)
+            action = ss::root_plan(root_q, env.n_choices(a, root_choice),
+                                   [&](int i) { return env.action(root_choice, i); }, rng);
         rng.store(a.rng + (int64_t)tree * B2_PCG64_STATE_WORDS);
         a.plan[tree] = (int8_t)action;
         int32_t* res = a.result + (int64_t)tree * B2_SPARSE_SAMPLING_RESULT_WORDS;

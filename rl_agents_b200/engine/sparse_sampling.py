@@ -29,7 +29,18 @@ def worst_case_nodes(n_actions, horizon, C):
     return sum(b ** d for d in range(horizon + 1)) + n_actions * sum(b ** d for d in range(horizon))
 
 
+def deterministic_nodes(n_actions, horizon):
+    """Nodes of a tree on a deterministic model in which every decision node has all n_actions actions: A^d decision
+    and A^d chance nodes at depth d >= 1, and the root."""
+    return 1 + 2 * sum(n_actions ** d for d in range(1, horizon + 1))
+
+
 class SparseSamplingEngine(TreeEngine):
+    """One tree per lane (finite MDPs) or per 16-lane group (HighwayLite), n_trees independent decisions per launch,
+    each a depth-first search (b2_sparse_sampling_plan)."""
+    WORKSPACE_BYTES = "b2_sparse_sampling_workspace_bytes"
+    PLAN = "b2_sparse_sampling_plan"
+
     def __init__(self, env_kind, n_trees, n_actions, horizon, C, gamma, mdp=None, record_tree=False, capacity=None,
                  device="cuda"):
         """record_tree: also dump every tree in creation order (capacity: nodes per tree, by default the worst
@@ -45,12 +56,12 @@ class SparseSamplingEngine(TreeEngine):
         self.tables = SampledFiniteTables(mdp, self.device) if env_kind == _lib.ENV_FINITE else None
         self.cfg = _lib.SparseSamplingConfig(env_kind, self.n_trees, self.n_actions, self.horizon, self.C, 0,
                                              self.gamma, self.tables.struct() if self.tables else _lib.FiniteMDPSampled())
-        self.workspace = torch.empty(int(self.lib.b2_sparse_sampling_workspace_bytes(self.cfg)), dtype=torch.uint8,
+        self._check_config()
+        self.workspace = torch.empty(int(getattr(self.lib, self.WORKSPACE_BYTES)(self.cfg)), dtype=torch.uint8,
                                      device=self.device)
         self.tree = None
         if record_tree:
-            self.capacity = int(capacity) if capacity is not None else worst_case_nodes(self.n_actions, self.horizon,
-                                                                                        self.C)
+            self.capacity = int(capacity) if capacity is not None else self.worst_case_nodes()
             if self.capacity >= 2 ** 31:
                 raise ValueError("a recorded tree of up to %d nodes does not fit int32 node ids" % self.capacity)
             self.tree = _lib.SparseSamplingTree(self.capacity, 0,
@@ -58,12 +69,19 @@ class SparseSamplingEngine(TreeEngine):
         self.root_q = torch.empty((self.n_trees, self.n_actions), dtype=torch.float64, device=self.device)
         self.plan_buf = torch.empty(self.n_trees, dtype=torch.int8, device=self.device)
 
+    def _check_config(self):
+        """Refuse what this engine's kernel cannot plan (the lane kernel plans every model)."""
+
+    def worst_case_nodes(self):
+        """The default dump capacity."""
+        return worst_case_nodes(self.n_actions, self.horizon, self.C)
+
     def plan(self, root_states, rng_words):
         """root_states: [n_trees] state ids (finite) or [n_trees, 136] words (HighwayLite), on the device."""
         self._load_rng(rng_words)
-        _lib.check(self.lib.b2_sparse_sampling_plan(self.cfg, _lib.ptr(root_states), self.tree, _lib.ptr(self.workspace),
-                                                    _lib.ptr(self.rng), _lib.ptr(self.root_q), _lib.ptr(self.plan_buf),
-                                                    _lib.ptr(self.result), _lib.current_stream()))
+        _lib.check(getattr(self.lib, self.PLAN)(self.cfg, _lib.ptr(root_states), self.tree, _lib.ptr(self.workspace),
+                                                _lib.ptr(self.rng), _lib.ptr(self.root_q), _lib.ptr(self.plan_buf),
+                                                _lib.ptr(self.result), _lib.current_stream()))
 
     def _check(self, res):
         """A sampled probability row that Generator.choice rejects raises its ValueError, as the reference's env step
@@ -82,3 +100,32 @@ class SparseSamplingEngine(TreeEngine):
             raise ValueError("the engine was built without record_tree")
         n = int(self.result[tree, 0].item())
         return {k: getattr(self, k)[tree, :n].cpu().numpy() for k in _lib.SPARSE_SAMPLING_TREE_FIELDS}
+
+
+def level_workspace_bytes(env_kind, n_actions, horizon, C):
+    """Bytes of workspace SparseSamplingLevelEngine allocates for one decision (None: the worst-case tree does not
+    fit int32 node ids)."""
+    cfg = _lib.SparseSamplingConfig(env_kind, 1, int(n_actions), int(horizon), int(C), 0, 0.0, _lib.FiniteMDPSampled())
+    n = int(_lib.load().b2_sparse_sampling_levels_workspace_bytes(cfg))
+    return n if n > 0 else None
+
+
+class SparseSamplingLevelEngine(SparseSamplingEngine):
+    """ONE decision on a deterministic model (HighwayLite, or a finite MDP in mode "deterministic") searched by the
+    whole GPU level by level (b2_sparse_sampling_plan_levels): the same outputs as SparseSamplingEngine bit for bit.
+    Its workspace is sized for the tree in which every decision node has all actions (level_workspace_bytes)."""
+    WORKSPACE_BYTES = "b2_sparse_sampling_levels_workspace_bytes"
+    PLAN = "b2_sparse_sampling_plan_levels"
+
+    def _check_config(self):
+        if self.n_trees != 1:
+            raise ValueError("the level-synchronous engine plans one decision (n_trees = 1, got %d)" % self.n_trees)
+        if self.tables is not None and self.tables.n_next != 1:
+            raise ValueError("the level-synchronous engine needs a deterministic model (finite MDP mode %r)"
+                             % self.tables.mode)
+        if level_workspace_bytes(self.env_kind, self.n_actions, self.horizon, self.C) is None:
+            raise ValueError("a sparse-sampling tree of horizon %d over %d actions does not fit int32 node ids"
+                             % (self.horizon, self.n_actions))
+
+    def worst_case_nodes(self):
+        return deterministic_nodes(self.n_actions, self.horizon)
