@@ -17,7 +17,7 @@ static float DT, KP_A, KP_HEADING, KP_LATERAL, PI_F, TWO_PI, HALF_PI, QUARTER_PI
 static float ASIN_C[10], SIN_C[5], COS_C[6];
 static int g_init = 0;
 
-static void hl_init(void) {
+void hl_init(void) {
     if (g_init) return;
     volatile float one = 1.0f;
     DT = one / 15.0f;
@@ -51,9 +51,9 @@ static float poly(float z, const float* c, int n) {
 }
 static float clampf(float x, float lo, float hi) { return fminf(fmaxf(x, lo), hi); }
 static float asin_p(float u) { const float z = u * u; return u * (1.0f + z * poly(z, ASIN_C, 10)); }
-static float sin_p(float x) { x = clampf(x, -HALF_PI, HALF_PI); const float z = x * x; return x * (1.0f + z * poly(z, SIN_C, 5)); }
-static float cos_p(float x) { x = clampf(x, -HALF_PI, HALF_PI); const float z = x * x; return 1.0f + z * poly(z, COS_C, 6); }
-static float not_zero(float x) { return fabsf(x) > EPS ? x : (x >= 0.0f ? EPS : -EPS); }
+float sin_p(float x) { x = clampf(x, -HALF_PI, HALF_PI); const float z = x * x; return x * (1.0f + z * poly(z, SIN_C, 5)); }
+float cos_p(float x) { x = clampf(x, -HALF_PI, HALF_PI); const float z = x * x; return 1.0f + z * poly(z, COS_C, 6); }
+float not_zero(float x) { return fabsf(x) > EPS ? x : (x >= 0.0f ? EPS : -EPS); }
 static int lane_of(float y) { return (int)clampf(rintf(y / LANE_W), 0.0f, (float)(HL_LANES - 1)); }
 
 static float idm(float v, float ts, int has_front, float x, float xf, float vf) {

@@ -19,4 +19,11 @@ typedef struct {
 int hl_available_actions(const hl_state* s, int* actions);   /* children order; returns the count */
 /* one decision step in place; returns the reward; *flags: bit0 terminated, bit1 truncated */
 float hl_step(hl_state* s, int action, int* flags);
+
+/* shared with the IntersectionLite statement (intersection_lite.c): the spec's polynomials sin_p / cos_p and
+ * not_zero, whose constants hl_init builds once (every exported entry point calls it) */
+void hl_init(void);
+float sin_p(float x);
+float cos_p(float x);
+float not_zero(float x);
 #endif

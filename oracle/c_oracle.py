@@ -1,6 +1,8 @@
 """ctypes wrapper of the C oracle (oracle/c) -- TEST INFRASTRUCTURE.  Third statement of the
 HighwayLite spec and a literal C OPD; pinned bit-exactly against oracle/envs.py and
-oracle/planners.py (tests/test_c_oracle.py), hence against the reference's golden vectors."""
+oracle/planners.py (tests/test_c_oracle.py), hence against the reference's golden vectors.  Also the
+third statement of the IntersectionLite spec (`il_*`), pinned against oracle/intersection.py and the
+same planners (tests/test_intersection_scene_families.py)."""
 import ctypes
 import os
 import subprocess
@@ -13,7 +15,8 @@ _lib = None
 
 
 def build(force=False):
-    srcs = [os.path.join(HERE, f) for f in ("highway_lite.c", "opd.c", "mcts.c", "highway_lite.h", "Makefile")]
+    srcs = [os.path.join(HERE, f) for f in ("highway_lite.c", "intersection_lite.c", "opd.c", "mcts.c", "highway_lite.h",
+                                               "intersection_lite.h", "Makefile")]
     if force or not os.path.exists(LIB) or any(os.path.getmtime(s) > os.path.getmtime(LIB) for s in srcs):
         subprocess.run(["make", "-C", HERE, "-s", "-B"], check=True)
     return LIB
@@ -26,6 +29,8 @@ def load():
         _lib = ctypes.CDLL(LIB)
         _lib.opd_highway_plan.restype = ctypes.c_int
         _lib.opd_highway_plan_wave.restype = ctypes.c_int
+        _lib.il_opd_plan.restype = ctypes.c_int
+        _lib.il_opd_plan_wave.restype = ctypes.c_int
         _lib.mcts_highway_plan.restype = ctypes.c_int
         _lib.mcts_highway_plan_wave.restype = ctypes.c_int
         _lib.hl_ttc_value_iteration.restype = ctypes.c_int
@@ -36,30 +41,40 @@ def _p(a):
     return a.ctypes.data_as(ctypes.c_void_p)
 
 
-def step_batch(words, actions):
-    """words [n,136] int32 (updated copy returned), actions [n] -> (words, rewards f32, flags)."""
-    lib = load()
+def _step_batch(fn, words, actions):
     w = np.ascontiguousarray(words, dtype=np.int32).copy()
     a = np.ascontiguousarray(actions, dtype=np.int32)
     r = np.zeros(len(a), dtype=np.float32)
     f = np.zeros(len(a), dtype=np.int32)
-    lib.hl_step_batch(_p(w), _p(a), _p(r), _p(f), ctypes.c_int(len(a)))
+    fn(_p(w), _p(a), _p(r), _p(f), ctypes.c_int(len(a)))
     return w, r, f
 
 
-def opd_plan(root_words, budget, gamma, terminal_reward=0.0):
-    """Returns a dict of node arrays in creation order (same fields as oracle.planners.Tree)."""
-    lib = load()
-    cap = 1 + (int(budget) // 5) * 5
+def step_batch(words, actions):
+    """words [n,136] int32 (updated copy returned), actions [n] -> (words, rewards f32, flags)."""
+    return _step_batch(load().hl_step_batch, words, actions)
+
+
+def il_step_batch(words, actions):
+    """IntersectionLite: words [n,136] int32 (updated copy returned), actions [n] -> (words, rewards f32, flags
+    (bit0 terminated, bit1 truncated))."""
+    return _step_batch(load().il_step_batch, words, actions)
+
+
+def _tree_arrays(cap):
     i32 = {k: np.zeros(cap, dtype=np.int32) for k in ("parent", "action", "depth", "count", "first_child",
                                                       "n_children", "done")}
     f64 = {k: np.zeros(cap, dtype=np.float64) for k in ("reward", "lower", "upper")}
+    ptrs = [_p(i32[k]) for k in ("parent", "action", "depth", "count", "first_child", "n_children", "done")]
+    return i32, f64, ptrs + [_p(f64["reward"]), _p(f64["lower"]), _p(f64["upper"])]
+
+
+def _strict(fn, n_actions, root_words, budget, gamma, terminal_reward):
+    i32, f64, ptrs = _tree_arrays(1 + (int(budget) // n_actions) * n_actions)
     n_leaves = ctypes.c_int32(0)
     root = np.ascontiguousarray(root_words, dtype=np.int32)
-    n = lib.opd_highway_plan(_p(root), ctypes.c_int(int(budget)), ctypes.c_double(gamma), ctypes.c_double(terminal_reward),
-                             _p(i32["parent"]), _p(i32["action"]), _p(i32["depth"]), _p(i32["count"]),
-                             _p(i32["first_child"]), _p(i32["n_children"]), _p(i32["done"]), _p(f64["reward"]),
-                             _p(f64["lower"]), _p(f64["upper"]), ctypes.byref(n_leaves))
+    n = fn(_p(root), ctypes.c_int(int(budget)), ctypes.c_double(gamma), ctypes.c_double(terminal_reward), *ptrs,
+           ctypes.byref(n_leaves))
     if n < 0:
         raise ValueError("This planner assumes that all rewards are normalized in [0, 1]")
     out = {k: v[:n] for k, v in {**i32, **f64}.items()}
@@ -67,25 +82,42 @@ def opd_plan(root_words, budget, gamma, terminal_reward=0.0):
     return out
 
 
-def opd_plan_wave(root_words, budget, gamma, width, terminal_reward=0.0, lag=0):
-    """The wavefront specification (oracle.planners.opd_plan_wavefront) in C; same dict as opd_plan + n_waves."""
-    lib = load()
-    cap = 1 + (int(budget) // 5) * 5
-    i32 = {k: np.zeros(cap, dtype=np.int32) for k in ("parent", "action", "depth", "count", "first_child",
-                                                      "n_children", "done")}
-    f64 = {k: np.zeros(cap, dtype=np.float64) for k in ("reward", "lower", "upper")}
+def _wave(fn, n_actions, root_words, budget, gamma, width, terminal_reward, lag, wave_end=None):
+    i32, f64, ptrs = _tree_arrays(1 + (int(budget) // n_actions) * n_actions)
     n_leaves, n_waves = ctypes.c_int32(0), ctypes.c_int32(0)
     root = np.ascontiguousarray(root_words, dtype=np.int32)
-    n = lib.opd_highway_plan_wave(_p(root), ctypes.c_int(int(budget)), ctypes.c_double(gamma),
-                                  ctypes.c_double(terminal_reward), ctypes.c_int(int(width)), ctypes.c_int(int(lag)),
-                                  _p(i32["parent"]), _p(i32["action"]), _p(i32["depth"]), _p(i32["count"]),
-                                  _p(i32["first_child"]), _p(i32["n_children"]), _p(i32["done"]), _p(f64["reward"]),
-                                  _p(f64["lower"]), _p(f64["upper"]), ctypes.byref(n_leaves), ctypes.byref(n_waves))
+    extra = [] if wave_end is None else [_p(wave_end)]
+    n = fn(_p(root), ctypes.c_int(int(budget)), ctypes.c_double(gamma), ctypes.c_double(terminal_reward),
+           ctypes.c_int(int(width)), ctypes.c_int(int(lag)), *ptrs, ctypes.byref(n_leaves), ctypes.byref(n_waves), *extra)
     if n < 0:
         raise ValueError("This planner assumes that all rewards are normalized in [0, 1]")
     out = {k: v[:n] for k, v in {**i32, **f64}.items()}
     out["n_leaves"], out["n_waves"] = n_leaves.value, n_waves.value
+    if wave_end is not None:
+        out["wave_end"] = wave_end[:n_waves.value].copy()
     return out
+
+
+def opd_plan(root_words, budget, gamma, terminal_reward=0.0):
+    """Returns a dict of node arrays in creation order (same fields as oracle.planners.Tree)."""
+    return _strict(load().opd_highway_plan, 5, root_words, budget, gamma, terminal_reward)
+
+
+def opd_plan_wave(root_words, budget, gamma, width, terminal_reward=0.0, lag=0):
+    """The wavefront specification (oracle.planners.opd_plan_wavefront) in C; same dict as opd_plan + n_waves."""
+    return _wave(load().opd_highway_plan_wave, 5, root_words, budget, gamma, width, terminal_reward, lag)
+
+
+def il_opd_plan(root_words, budget, gamma, terminal_reward=0.0):
+    """OPD on an IntersectionLite scene (3 actions); the same dict as opd_plan."""
+    return _strict(load().il_opd_plan, 3, root_words, budget, gamma, terminal_reward)
+
+
+def il_opd_plan_wave(root_words, budget, gamma, width, terminal_reward=0.0, lag=0):
+    """The wavefront specification on an IntersectionLite scene; the same dict as opd_plan_wave, plus `wave_end`:
+    per wave, the number of nodes after it (wave w created the ids wave_end[w - 1] .. wave_end[w] - 1)."""
+    wave_end = np.zeros(1 + int(budget) // 3, dtype=np.int32)
+    return _wave(load().il_opd_plan_wave, 3, root_words, budget, gamma, width, terminal_reward, lag, wave_end)
 
 
 def mcts_plan(root_words, episodes, horizon, gamma, temperature, rng_words):

@@ -144,8 +144,12 @@ def _idm(v, has_front, d, v_f):
     return np.where(has_front, acc - COMFORT_ACC_MAX * (q * q), acc).astype(f32)
 
 
-def intersection_step(st, action):
-    """One decision step in place; returns (reward f32, terminated, truncated)."""
+def intersection_step(st, action, on_substep=None):
+    """One decision step in place; returns (reward f32, terminated, truncated).  `on_substep` (tests' path census)
+    is called after every sub-step with keyword arguments: sub, present (at the sub-step's start), s_front (the
+    candidate fronts' s, inf elsewhere), has_front, yields, lane, hit (pair matrices), arrived_now (the ego reached
+    its route's end), left (others that left), spawn (None, or a dict of the spawn's route, clear, free slots, slot
+    and the spawn_seq it used); it does not touch the step."""
     n = V_SLOTS
     if action == A_FASTER:
         st.speed_index = min(st.speed_index + 1, 2)
@@ -153,8 +157,8 @@ def intersection_step(st, action):
         st.speed_index = max(st.speed_index - 1, 0)
     ts0 = f32(SPEED_STEP * f32(st.speed_index))
     idx = np.arange(n)
-    for _ in range(SUBSTEPS):
-        present = (st.flags & 1) != 0
+    for sub in range(SUBSTEPS):
+        present = present0 = (st.flags & 1) != 0
         crashed = (st.flags & 2) != 0
         entry = st.route // 3
         turn = st.route % 3
@@ -196,11 +200,13 @@ def intersection_step(st, action):
         # ---- vehicles leave at the end of their route (the ego: arrived) ----
         length = np.array([LEN[t] for t in turn], f32)
         gone = present & (st.s >= length)
+        arrived_now = bool(gone[0])
         if gone[0]:
             st.arrived = 1
         gone[0] = False
         st.flags = np.where(gone, 0, st.flags).astype(np.int32)
         # ---- deterministic spawning ----
+        spawn = None
         st.spawn_clock += 1
         if st.spawn_clock >= SPAWN_PERIOD:
             st.spawn_clock = 0
@@ -211,9 +217,13 @@ def intersection_step(st, action):
             present = (st.flags & 1) != 0
             clear = not np.any(present & (st.route // 3 == route // 3) & (st.s < ENTRY_CLEAR))
             free = np.nonzero(~present[1:])[0]
-            if clear and free.size:
-                slot = 1 + int(free[0])
+            slot = 1 + int(free[0]) if clear and free.size else -1
+            if slot > 0:
                 st.s[slot], st.v[slot], st.route[slot], st.flags[slot] = f32(0.0), SPAWN_SPEED, route, 1
+            spawn = {"route": route, "clear": clear, "free": 1 + free, "slot": slot, "seq": k}
+        if on_substep is not None:
+            on_substep(sub=sub, present=present0, s_front=s_f, has_front=has_f, yields=yields, lane=lane, hit=hit,
+                       arrived_now=arrived_now, left=gone, spawn=spawn)
     st.t += 1
     crashed0 = bool(st.flags[0] & 2)
     if crashed0:
