@@ -23,7 +23,6 @@ def main():
     ap.add_argument("--sweeps", type=int, default=100)
     ap.add_argument("--mode", default="sparse", choices=["sparse", "deterministic"])
     ap.add_argument("--cpu-sweeps", type=int, default=3)
-    ap.add_argument("--kernel", type=int, default=0, help="0 auto, 1 plain tiled, 2 TMA-staged")
     a = ap.parse_args()
     import torch
     import torch.distributed as dist
@@ -50,7 +49,6 @@ def main():
         T = rng.integers(0, S, size=(rows, A), dtype=np.int64)
         eng = VIEngine("deterministic", T, R, term, gamma=0.95, device=dev, row_begin=b, row_end=e, n_states=S)
         P = N = None
-    eng.problem.reserved = a.kernel
     eng.problem.rtol = 0.0                               # timing run: never converge early (SURVEY 8d)
     eng.problem.atol = -1.0
 

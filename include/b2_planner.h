@@ -103,8 +103,7 @@ typedef struct b2_vi_problem {
     int32_t mode;
     int32_t n_actions;   /* A                                                */
     int32_t n_next;      /* B (sparse), S (stochastic), ignored otherwise    */
-    int32_t reserved;    /* kernel choice: 0 auto (register kernel when the shape
-                            allows, else tiled), 1 tiled, 2 TMA-staged tiled    */
+    int32_t reserved;    /* must be 0                                        */
     int64_t n_states;    /* S of the whole MDP (length of V)                 */
     int64_t row_begin;   /* state slab [row_begin, row_end) owned by the call */
     int64_t row_end;
@@ -190,10 +189,7 @@ typedef struct b2_opd_config {
     int32_t node_capacity;  /* per tree, >= 1 + n_expansions * n_actions     */
     int32_t plan_capacity;  /* per tree, >= n_expansions + 1                 */
     int32_t keys_in_smem;   /* 1: frontier keys in shared memory when they fit */
-    int32_t reserved;       /* HighwayLite batch kernel: 0 default (8 trees per CTA, packed
-                               slots, block barriers between the phases), 1 one tree per warp,
-                               2 8 trees per CTA as a dataflow over a work ring in shared
-                               memory (no block barriers); identical trees, 0 is fastest */
+    int32_t reserved;       /* must be 0                                     */
     double terminal_reward; /* config["terminal_reward"] (:60-63)            */
     const double* gamma_pow;     /* [n_expansions+2] gamma**d   (host floats) */
     const double* gamma_pow_div; /* [n_expansions+2] gamma**d / (1 - gamma)   */
@@ -355,7 +351,8 @@ typedef struct b2_opd_handle b2_opd_handle;
 typedef struct b2_opd_host_config {
     int32_t env_kind, n_trees, n_actions;
     int32_t budget;          /* config["budget"]; n_expansions = budget / n_actions (:118) */
-    int32_t keys_in_smem, kernel;
+    int32_t keys_in_smem;
+    int32_t kernel;          /* copied to b2_opd_config.reserved: must be 0         */
     double gamma;            /* config["gamma"], 0 <= gamma < 1                     */
     double terminal_reward;
     b2_finite_mdp mdp;       /* HOST tables when env_kind == B2_ENV_FINITE          */

@@ -448,271 +448,6 @@ __global__ void __launch_bounds__(MT_THREADS, B2_MT_MIN_BLOCKS) opd_highway_mult
 }
 
 // ---------------------------------------------------------------------------
-// HighwayLite, batched, DATAFLOW variant of the kernel above (b2_opd_config.reserved = 2): the same 8 trees per CTA
-// and the same packing of children onto half-warp groups, but no block barrier inside the search.  The children of
-// an expansion are work items on a ring in shared memory; every warp pops up to two items (of any trees) and
-// simulates them; the group that simulates the LAST outstanding child of a tree (its atomic decrement of the tree's
-// pending count returns 1) makes its warp commit that expansion, select the tree's next leaf and push the new
-// children at once.  Trees therefore run ahead of each other: no warp waits for the slowest warp of a round, a
-// half-filled third round does not stall the CTA, and select / commit of one tree overlap the simulations of the
-// others.  Every tree still performs select -> children -> commit strictly in order, so trees are bit-identical
-// with the barrier version.
-// Synchronisation: ring and counters in shared memory, ring guarded by a spin lock taken by lane 0; data handed from
-// warp to warp (node records in shared memory; scenes, tree arrays and tournament levels in global memory, same SM)
-// is published with __threadfence_block() before the counter decrement / lock release and read after the matching
-// acquire.  Idle polling is bounded: a warp that polls FLOW_SPIN_LIMIT times without finding work gives up and
-// flags error 3.
-// ---------------------------------------------------------------------------
-constexpr int FLOW_Q = 64;                  // ring capacity (outstanding children <= MT_TREES * MAX_BRANCH = 64)
-constexpr int FLOW_SPIN_LIMIT = 1 << 22;
-
-struct FlowShared {
-    Shared sh[MT_TREES];
-    int n[MT_TREES], mask[MT_TREES], c0[MT_TREES];    // current expansion of every tree
-    int pending[MT_TREES];                             // its children not simulated yet
-    int n_nodes[MT_TREES], max_depth[MT_TREES], term_exp[MT_TREES], n_exp[MT_TREES];
-    int queue[FLOW_Q];                                 // work items: tree << 4 | child
-    int head, tail, lock, live, stuck;
-};
-
-__device__ __forceinline__ void flow_lock(int* lock) {
-    while (atomicCAS(lock, 0, 1) != 0) {}
-    __threadfence_block();
-}
-__device__ __forceinline__ void flow_unlock(int* lock) {
-    __threadfence_block();
-    atomicExch(lock, 0);
-}
-
-struct FlowTree {       // what a warp needs to work on tree `tr` of the CTA
-    Tournament T;
-    int64_t nb;
-    int32_t* exp_order;
-};
-
-__device__ __forceinline__ void flow_tree(const OpdArgs& a, int tree0, int tr, double* smem_d, FlowTree& ft) {
-    const int tree = tree0 + tr;
-    ft.nb = (int64_t)tree * a.cfg.node_capacity;
-    char* ws = a.workspace + (int64_t)tree * a.lay.ws_bytes_per_tree;
-    setup_tournament(ft.T, a.lay, smem_d + (size_t)tr * a.lay.smem_doubles, (double*)ws);
-    ft.exp_order = (int32_t*)(ws + a.lay.ws_doubles * 8);
-}
-
-// select the next leaf of tree `tr` and push its children on the ring (warp-collective)
-__device__ __forceinline__ void flow_select_publish(const OpdArgs& a, FlowShared& fs, FlowTree& ft, int tr, int lane) {
-    const int leaf = ft.T.select(lane);
-    if (lane == 0) {
-        Shared& sh = fs.sh[tr];
-        sh.leaf = leaf;
-        sh.depth = a.tree.depth[ft.nb + leaf];
-        sh.lower = a.tree.lower[ft.nb + leaf];
-        sh.done_parent = (a.tree.meta[ft.nb + leaf] >> 16) & 1;
-        const volatile int32_t* w = a.tree.state + (ft.nb + leaf) * hw::WORDS;
-        const int mask = hw::avail_mask(__int_as_float(w[hw::V]), w[8 * hw::V + 1]);
-        const int n = __popc(mask);
-        fs.mask[tr] = mask;
-        fs.n[tr] = n;
-        fs.c0[tr] = fs.n_nodes[tr];
-        fs.pending[tr] = n;
-        flow_lock(&fs.lock);            // (its fences publish the record above together with the items)
-        const int t = fs.tail;
-        for (int k = 0; k < n; ++k) fs.queue[(t + k) & (FLOW_Q - 1)] = (tr << 4) | k;
-        *(volatile int*)&fs.tail = t + n;
-        flow_unlock(&fs.lock);
-    }
-    __syncwarp();
-}
-
-// all children of tree `tr`'s expansion are simulated: commit it, then go on with the tree (warp-collective)
-__device__ __forceinline__ void flow_commit(const OpdArgs& a, FlowShared& fs, int tree0, int tr, double* smem_d, int lane) {
-    __threadfence_block();          // acquire: the children's records
-    FlowTree ft;
-    flow_tree(a, tree0, tr, smem_d, ft);
-    Shared& sh = fs.sh[tr];
-    const int n = fs.n[tr], c0 = fs.n_nodes[tr];
-    commit_expansion(a, ft.T, sh, ft.nb, sh.leaf, c0, n, fs.n_exp[tr], ft.exp_order, lane);
-    __syncwarp();
-    int fin = 0;
-    if (lane == 0) {
-        fs.term_exp[tr] += sh.done_parent;
-        fs.max_depth[tr] = max(fs.max_depth[tr], sh.depth + 1);
-        fs.n_nodes[tr] = c0 + n;
-        fs.n_exp[tr] += 1;
-        fin = (sh.error != 0 || fs.n_exp[tr] >= a.cfg.n_expansions) ? 1 : 0;     // deterministic.py:46-47 raises
-        if (fin) { __threadfence_block(); atomicSub(&fs.live, 1); }
-    }
-    fin = __shfl_sync(0xffffffffu, fin, 0);
-    if (__all_sync(0xffffffffu, fin == 0)) flow_select_publish(a, fs, ft, tr, lane);
-}
-
-__global__ void __launch_bounds__(MT_THREADS, B2_MT_MIN_BLOCKS) opd_highway_flow_kernel(OpdArgs a) {
-    extern __shared__ double smem_d[];
-    __shared__ FlowShared fs;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, li = tid & 15, half = (tid >> 4) & 1;
-    int grp = tid >> 4;
-    asm volatile("" : "+r"(grp));
-    const int tree0 = blockIdx.x * MT_TREES;
-    const int n_local = min(MT_TREES, a.cfg.n_trees - tree0);
-    const bool owner = __all_sync(0xffffffffu, warp < n_local);
-    if (lane == 0) {
-        fs.sh[warp].error = 0;
-        fs.n[warp] = 0; fs.pending[warp] = 0;
-        fs.n_nodes[warp] = 1; fs.max_depth[warp] = 0; fs.term_exp[warp] = 0; fs.n_exp[warp] = 0;
-    }
-    if (tid == 0) { fs.head = 0; fs.tail = 0; fs.lock = 0; fs.stuck = 0; fs.live = a.cfg.n_expansions > 0 ? n_local : 0; }
-    if (owner) {
-        FlowTree ft;
-        flow_tree(a, tree0, warp, smem_d, ft);
-        init_tree(a, ft.T, ft.nb, lane, 32);
-        int32_t* st = a.tree.state + ft.nb * hw::WORDS;
-        for (int i = lane; i < hw::WORDS; i += 32) st[i] = a.root_states[(int64_t)(tree0 + warp) * hw::WORDS + i];
-    }
-    __syncthreads();
-    if (owner && a.cfg.n_expansions > 0) {      // first expansion of the warp's own tree
-        FlowTree ft;
-        flow_tree(a, tree0, warp, smem_d, ft);
-        flow_select_publish(a, fs, ft, warp, lane);
-    }
-    int spins = 0;
-    while (true) {
-        // ---- pop up to two children (of any trees) ----
-        int item0 = -1, item1 = -1;
-        if (lane == 0 && *(volatile int*)&fs.tail != *(volatile int*)&fs.head) {
-            flow_lock(&fs.lock);
-            const int h = fs.head, avail = fs.tail - h;
-            if (avail > 0) item0 = fs.queue[h & (FLOW_Q - 1)];
-            if (avail > 1) item1 = fs.queue[(h + 1) & (FLOW_Q - 1)];
-            *(volatile int*)&fs.head = h + min(avail, 2);
-            flow_unlock(&fs.lock);
-        }
-        item0 = __shfl_sync(0xffffffffu, item0, 0);
-        item1 = __shfl_sync(0xffffffffu, item1, 0);
-        __syncwarp();                           // lane 0's acquire ordered before the other lanes' reads below
-        if (__all_sync(0xffffffffu, item0 >= 0)) {
-            spins = 0;
-            const int item = half ? item1 : item0;
-            const bool real = item >= 0;
-            const int tr = (real ? item : item0) >> 4, k = real ? item & 15 : 0;
-            const int64_t nb = (int64_t)(tree0 + tr) * a.cfg.node_capacity;
-            int32_t* states = a.tree.state + nb * hw::WORDS;
-            hw::Lane L;
-            int t, si;
-            hw::load_state(states + (int64_t)fs.sh[tr].leaf * hw::WORDS, li, L, t, si);
-            const int action = real ? hw::nth_action(fs.mask[tr], k) : hw::A_IDLE;
-            bool term, trunc;
-            const float r = hw::step(L, li, t, si, action, term, trunc, 0xffffffffu);
-            if (real) {
-                hw::store_state(states + (int64_t)(fs.c0[tr] + k) * hw::WORDS, li, L, t, si);
-                if (li == 0) {
-                    fs.sh[tr].child_reward[k] = (double)r;
-                    fs.sh[tr].child_done[k] = term ? 1 : 0;
-                    fs.sh[tr].child_action[k] = action;
-                }
-            }
-            __threadfence_block();              // release: child scene (global) and record (shared) ...
-            __syncwarp();                       // ... of every lane of the group, before the count drops
-            int last = 0;                       // did my group simulate the last outstanding child of its tree?
-            if (real && li == 0) last = atomicSub(&fs.pending[tr], 1) == 1 ? 1 : 0;
-            const int last0 = __shfl_sync(0xffffffffu, last, 0), last1 = __shfl_sync(0xffffffffu, last, 16);
-            const int tr0 = item0 >> 4, tr1 = (item1 >= 0 ? item1 : item0) >> 4;
-            if (__all_sync(0xffffffffu, last0 != 0)) flow_commit(a, fs, tree0, tr0, smem_d, lane);
-            if (__all_sync(0xffffffffu, last1 != 0)) flow_commit(a, fs, tree0, tr1, smem_d, lane);
-        } else {
-            int live = 0, stuck = 0;
-            if (lane == 0) { live = *(volatile int*)&fs.live; stuck = *(volatile int*)&fs.stuck; }
-            live = __shfl_sync(0xffffffffu, live, 0);
-            stuck = __shfl_sync(0xffffffffu, stuck, 0);
-            if (__all_sync(0xffffffffu, live == 0 || stuck != 0)) break;
-            ++spins;
-            __nanosleep(64);
-            if (__all_sync(0xffffffffu, spins > FLOW_SPIN_LIMIT)) {
-                if (lane == 0) { fs.stuck = 1; fs.sh[warp].error = 3; }
-                break;
-            }
-        }
-    }
-    __syncthreads();            // every commit of every tree is done (and visible) before the bottom-up passes
-    if (owner) {
-        FlowTree ft;
-        flow_tree(a, tree0, warp, smem_d, ft);
-        finish_tree(a, ft.nb, tree0 + warp, fs.n_nodes[warp], fs.n_exp[warp], fs.max_depth[warp], fs.term_exp[warp],
-                    fs.sh[warp].error, ft.exp_order, lane);
-    }
-}
-
-// ---------------------------------------------------------------------------
-// HighwayLite, batched, warp-autonomous: one tree per WARP.  The warp selects,
-// simulates the children two at a time on its two 16-lane halves, commits and
-// finishes entirely on its own -- no block barrier, no coupling between trees, so
-// the warps of an SM drift apart and hide each other's select/commit latency.
-// ---------------------------------------------------------------------------
-constexpr int WT_WARPS = 4;
-
-#ifndef B2_WT_MIN_BLOCKS
-#define B2_WT_MIN_BLOCKS 6
-#endif
-__global__ void __launch_bounds__(WT_WARPS * 32, B2_WT_MIN_BLOCKS) opd_highway_warp_kernel(OpdArgs a) {
-    extern __shared__ double smem_d[];
-    __shared__ Shared shs[WT_WARPS];
-    const int tid = threadIdx.x, lane = tid & 31, li = tid & 15, half = (tid >> 4) & 1;
-    int warp = tid >> 5;
-    asm volatile("" : "+r"(warp));
-    const int tree_id = blockIdx.x * WT_WARPS + warp;
-    if (tree_id >= a.cfg.n_trees) return;        // whole warp; nothing below synchronises across warps
-    Shared& sh = shs[warp];
-    const int64_t nb = (int64_t)tree_id * a.cfg.node_capacity;
-    char* ws = a.workspace + (int64_t)tree_id * a.lay.ws_bytes_per_tree;
-    Tournament T;
-    setup_tournament(T, a.lay, smem_d + (size_t)warp * a.lay.smem_doubles, (double*)ws);
-    int32_t* exp_order = (int32_t*)(ws + a.lay.ws_doubles * 8);
-    int32_t* states = a.tree.state + nb * hw::WORDS;
-    init_tree(a, T, nb, lane, 32);
-    for (int i = lane; i < hw::WORDS; i += 32) states[i] = a.root_states[(int64_t)tree_id * hw::WORDS + i];
-    if (lane == 0) sh.error = 0;
-    __syncwarp();
-    int n_nodes = 1, max_depth = 0, term_exp = 0, it = 0;
-    for (; it < a.cfg.n_expansions; ++it) {
-        const int leaf = T.select(lane);
-        if (lane == 0) {
-            sh.depth = a.tree.depth[nb + leaf];
-            sh.lower = a.tree.lower[nb + leaf];
-            sh.done_parent = (a.tree.meta[nb + leaf] >> 16) & 1;
-        }
-        // "deep copy" of the parent scene into registers (both halves hold it)
-        hw::Lane P;
-        int pt, psi;
-        hw::load_state(states + (int64_t)leaf * hw::WORDS, li, P, pt, psi);
-        const int mask = hw::avail_mask(__shfl_sync(0xffffffffu, P.y, 0, 16), psi);
-        const int n = __popc(mask);
-        for (int base = 0; base < n; base += 2) {
-            const int k = base + half;
-            const bool real = k < n;
-            const int action = real ? hw::nth_action(mask, k) : hw::A_IDLE;
-            hw::Lane L = P;
-            int t = pt, si = psi;
-            bool term, trunc;
-            const float r = hw::step(L, li, t, si, action, term, trunc, 0xffffffffu);
-            if (real) {
-                hw::store_state(states + (int64_t)(n_nodes + k) * hw::WORDS, li, L, t, si);
-                if (li == 0) {
-                    sh.child_reward[k] = (double)r;
-                    sh.child_done[k] = term ? 1 : 0;
-                    sh.child_action[k] = action;
-                }
-            }
-        }
-        __syncwarp();
-        term_exp += sh.done_parent;
-        max_depth = max(max_depth, sh.depth + 1);
-        commit_expansion(a, T, sh, nb, leaf, n_nodes, n, it, exp_order, lane);
-        n_nodes += n;
-        __syncwarp();
-        if (sh.error) { ++it; break; }
-    }
-    finish_tree(a, nb, tree_id, n_nodes, it, max_depth, term_exp, sh.error, exp_order, lane);
-}
-
-// ---------------------------------------------------------------------------
 // batched env transition (b2_highway_step): one scene per 16-lane group
 // ---------------------------------------------------------------------------
 __global__ void __launch_bounds__(128) highway_step_kernel(int32_t* states, const int32_t* actions, float* reward,
@@ -854,6 +589,7 @@ extern "C" int64_t b2_opd_workspace_bytes(const b2_opd_config* cfg) {
 extern "C" int b2_opd_plan(const b2_opd_config* cfg, const int32_t* root_states, const b2_opd_tree* tree,
                            void* workspace, int8_t* plan, int32_t* result, void* stream_) {
     B2_REQUIRE(cfg && root_states && tree && workspace && plan && result, "null pointer");
+    B2_REQUIRE(cfg->reserved == 0, "b2_opd_config.reserved must be 0");
     B2_REQUIRE(cfg->n_trees > 0 && cfg->n_expansions >= 0, "bad batch / budget");
     B2_REQUIRE(cfg->n_actions > 0 && cfg->n_actions <= MAX_BRANCH, "n_actions must be in 1..8");
     B2_REQUIRE((int64_t)cfg->node_capacity >= 1 + (int64_t)cfg->n_expansions * cfg->n_actions, "node_capacity too small");
@@ -876,18 +612,7 @@ extern "C" int b2_opd_plan(const b2_opd_config* cfg, const int32_t* root_states,
     } else if (cfg->env_kind == B2_ENV_HIGHWAY) {
         B2_REQUIRE(cfg->n_actions == B2_HW_ACTIONS, "HighwayLite has 5 actions");
         const size_t smem_multi = smem * MT_TREES;
-        const size_t smem_warp = smem * WT_WARPS;
-        if (cfg->n_trees >= 2 * MT_TREES && smem_warp <= 32 * 1024 && cfg->reserved == 1) {
-            // batch mode, warp-autonomous: one tree per warp, no block barriers
-            B2_CUDA_CHECK(cudaFuncSetAttribute(opd_highway_warp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                               (int)smem_warp));
-            opd_highway_warp_kernel<<<(cfg->n_trees + WT_WARPS - 1) / WT_WARPS, WT_WARPS * 32, smem_warp, stream>>>(a);
-        } else if (cfg->n_trees >= 2 * MT_TREES && smem_multi <= 64 * 1024 && cfg->reserved == 2) {
-            // batch mode, dataflow: 8 trees per CTA, children on a shared work ring, no block barriers
-            B2_CUDA_CHECK(cudaFuncSetAttribute(opd_highway_flow_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                               (int)smem_multi));
-            opd_highway_flow_kernel<<<(cfg->n_trees + MT_TREES - 1) / MT_TREES, MT_THREADS, smem_multi, stream>>>(a);
-        } else if (cfg->n_trees >= 2 * MT_TREES && smem_multi <= 64 * 1024) {
+        if (cfg->n_trees >= 2 * MT_TREES && smem_multi <= 64 * 1024) {
             // batch mode: 8 trees per CTA, children packed densely on the simulation slots
             B2_CUDA_CHECK(cudaFuncSetAttribute(opd_highway_multi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                (int)smem_multi));

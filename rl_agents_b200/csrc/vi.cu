@@ -237,166 +237,10 @@ __global__ void __launch_bounds__(256) vi_sweep_row_kernel(SweepArgs g) {
     if ((threadIdx.x & 31) == 0 && bad) atomicAdd(g.viol + g.sweep, bad);
 }
 
-// ---------------------------------------------------------------------------
-// TMA-staged variant of the gather sweep (the default for well-formed shapes).
-// Persistent CTAs; a 3-stage ring of shared-memory tiles is filled by bulk async
-// copies (cp.async.bulk -> UBLKCP, completion on an mbarrier) issued by one
-// thread, so that the P / N / R / Q_old streams of the next two tiles are in
-// flight while the current tile's V gathers and reductions run.  Each thread
-// then has all of its gathers outstanding at once (indices come from shared
-// memory, not from a dependent global load).
-// ---------------------------------------------------------------------------
-constexpr int TMA_THREADS = 512;
-constexpr int TMA_STAGES = 3;
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, unsigned count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, unsigned bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, unsigned parity) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "WAIT_LOOP:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-        "@p bra DONE;\n\t"
-        "bra WAIT_LOOP;\n\t"
-        "DONE:\n\t}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, unsigned bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                     smem_u32(dst)),
-                 "l"(src), "r"(bytes), "r"(smem_u32(bar))
-                 : "memory");
-}
-
-struct TileLayout {   // byte offsets inside one stage
-    int p, n, r, q, t, bytes;
-};
-
-__global__ void __launch_bounds__(TMA_THREADS, 1) vi_sweep_tma_kernel(SweepArgs g, TileLayout lay) {
-    if (g.sweep > 0 && g.viol[g.sweep - 1] == 0) return;   // already converged
-    extern __shared__ __align__(128) unsigned char smem_raw[];
-    __shared__ uint64_t full_bar[TMA_STAGES];
-    const int tid = threadIdx.x;
-    const int A = g.A, B = g.B, E = A * B, TS = g.tile_states;
-    double* qs = (double*)(smem_raw + (size_t)TMA_STAGES * lay.bytes);
-    const int64_t n_tiles = (g.rows + TS - 1) / TS;
-    const int64_t my_tiles = blockIdx.x < n_tiles ? (n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-
-    auto issue = [&](int64_t k) {   // thread 0: bulk-load this CTA's k-th tile into stage k % STAGES
-        const int64_t tile = blockIdx.x + k * gridDim.x;
-        const int64_t s0 = tile * TS;
-        const int ns = (int)min((int64_t)TS, g.rows - s0);
-        unsigned char* st = smem_raw + (size_t)(k % TMA_STAGES) * lay.bytes;
-        uint64_t* bar = &full_bar[k % TMA_STAGES];
-        const unsigned bp = g.P ? (unsigned)ns * E * 8 : 0, bn = (unsigned)ns * E * 4, br = (unsigned)ns * A * 8,
-                       bt = (unsigned)ns;
-        mbar_expect_tx(bar, bp + bn + 2 * br + bt);
-        if (bp) bulk_g2s(st + lay.p, g.P + s0 * E, bp, bar);
-        bulk_g2s(st + lay.n, g.N + s0 * E, bn, bar);
-        bulk_g2s(st + lay.r, g.R + s0 * A, br, bar);
-        bulk_g2s(st + lay.q, g.q_old + s0 * A, br, bar);
-        bulk_g2s(st + lay.t, g.term + s0, bt, bar);
-    };
-
-    if (tid == 0) {
-        for (int s = 0; s < TMA_STAGES; ++s) mbar_init(&full_bar[s], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    if (tid == 0)
-        for (int64_t k = 0; k < my_tiles && k < TMA_STAGES; ++k) issue(k);
-
-    int bad = 0;
-    for (int64_t k = 0; k < my_tiles; ++k) {
-        const int64_t tile = blockIdx.x + k * gridDim.x;
-        const int64_t s0 = tile * TS;
-        const int ns = (int)min((int64_t)TS, g.rows - s0);
-        const int ne = ns * E;
-        unsigned char* st = smem_raw + (size_t)(k % TMA_STAGES) * lay.bytes;
-        double* sp = (double*)(st + lay.p);
-        const int32_t* sn = (const int32_t*)(st + lay.n);
-        const double* sr = (const double*)(st + lay.r);
-        const double* sq = (const double*)(st + lay.q);
-        const uint8_t* stt = (const uint8_t*)(st + lay.t);
-        mbar_wait(&full_bar[k % TMA_STAGES], (unsigned)((k / TMA_STAGES) & 1));
-        // phase 1: V gathers (all of a thread's gathers in flight), products in place
-        constexpr int U = 8;
-        for (int i0 = tid; i0 < ne; i0 += TMA_THREADS * U) {
-            double v[U];
-#pragma unroll
-            for (int u = 0; u < U; ++u) {
-                const int i = i0 + u * TMA_THREADS;
-                if (i < ne) v[u] = __ldg(g.v_in + sn[i]);
-            }
-#pragma unroll
-            for (int u = 0; u < U; ++u) {
-                const int i = i0 + u * TMA_THREADS;
-                if (i < ne) sp[i] = g.P ? sp[i] * v[u] : v[u];
-            }
-        }
-        __syncthreads();
-        // phase 2: one thread per (s,a)
-        const int nsa = ns * A;
-        for (int r = tid; r < nsa; r += TMA_THREADS) {
-            double nv = np_pairwise_sum([&](int i) { return sp[i]; }, r * B, B);
-            if (stt[r / A]) nv = 0.0;
-            const double q = sr[r] + g.gamma * nv;
-            if (!np_isclose(sq[r], q, g.rtol, g.atol)) bad++;
-            __stcs(g.q_new + s0 * A + r, q);
-            qs[r] = q;
-        }
-        __syncthreads();
-        // phase 3: V' = max_a Q'
-        for (int s = tid; s < ns; s += TMA_THREADS) {
-            double m = qs[s * A];
-            for (int a = 1; a < A; ++a) {
-                const double x = qs[s * A + a];
-                m = x > m ? x : m;
-            }
-            g.v_out[g.row_begin + s0 + s] = m;
-        }
-        __syncthreads();   // every generic-proxy access to this stage (and qs) is done
-        if (tid == 0 && k + TMA_STAGES < my_tiles) {
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            issue(k + TMA_STAGES);
-        }
-    }
-    bad = __reduce_add_sync(0xffffffffu, bad);
-    if ((tid & 31) == 0 && bad) atomicAdd(g.viol + g.sweep, bad);
-}
-
-// Dense stochastic mode: one thread per (s,a) row, numpy summation order.
-__global__ void __launch_bounds__(128) vi_sweep_dense_kernel(SweepArgs g) {
-    if (g.sweep > 0 && g.viol[g.sweep - 1] == 0) return;
-    extern __shared__ double smem[];   // q of the CTA's rows: [128]
-    const int tid = threadIdx.x;
-    const int64_t n_rows = g.rows * g.A;
-    // CTA covers 128 consecutive (s,a) rows; requires 128 % A == 0 or handles V by atomics-free pass below
-    const int64_t row = (int64_t)blockIdx.x * 128 + tid;
-    int bad = 0;
-    double q = 0.0;
-    if (row < n_rows) {
-        const double* p = g.P + row * (int64_t)g.B;
-        double nv = np_pairwise_sum([&](int i) { return p[i] * g.v_in[i]; }, 0, g.B);
-        const int64_t s = row / g.A;
-        if (g.term[s]) nv = 0.0;
-        q = g.R[row] + g.gamma * nv;
-        if (!np_isclose(g.q_old[row], q, g.rtol, g.atol)) bad = 1;
-        g.q_new[row] = q;
-    }
-    bad = __reduce_add_sync(0xffffffffu, bad);
-    if ((tid & 31) == 0 && bad) atomicAdd(g.viol + g.sweep, bad);
-}
-
 // Dense stochastic mode, cooperative: an 8-lane group per (s,a) row.  numpy's pairwise sum keeps eight strided
 // accumulators r[j] += a[i + j] over a block of <= 128 elements and combines them as
 // ((r0+r1)+(r2+r3))+((r4+r5)+(r6+r7)): lane j of the group IS accumulator j, so the row of P is read in
-// coalesced 64-byte pieces (the one-thread-per-row kernel reads with a stride of S doubles), and the fixed
+// coalesced 64-byte pieces (one thread per row would read with a stride of S doubles), and the fixed
 // combination tree is an xor-butterfly (fp addition commutes, so every lane ends with the same bits).
 // Blocks longer than 128 split in halves exactly as numpy does (n2 = n/2 rounded down to a multiple of 8).
 template <typename Load>
@@ -496,6 +340,7 @@ extern "C" int b2_vi_sweep(const b2_vi_problem* p, const double* v_in, const dou
     B2_REQUIRE(p->reward && p->transition && p->terminal, "MDP tables (reward / transition / terminal) missing");
     B2_REQUIRE(p->n_actions > 0 && p->row_end >= p->row_begin && p->row_end <= p->n_states, "bad shape");
     B2_REQUIRE(sweep_index >= 0, "sweep_index < 0");
+    B2_REQUIRE(p->reserved == 0, "b2_vi_problem.reserved must be 0");
     cudaStream_t stream = (cudaStream_t)stream_;
     SweepArgs g;
     g.R = p->reward; g.term = p->terminal; g.v_in = v_in; g.q_old = q_old; g.q_new = q_new; g.v_out = v_out;
@@ -506,10 +351,7 @@ extern "C" int b2_vi_sweep(const b2_vi_problem* p, const double* v_in, const dou
         B2_REQUIRE(p->n_next == p->n_states, "stochastic mode: n_next must equal n_states");
         g.P = (const double*)p->transition; g.N = nullptr; g.B = (int)p->n_states; g.tile_states = 0;
         const int64_t n_rows = g.rows * g.A;
-        if (p->reserved == 1)     // one thread per row (kept selectable; the group kernel is the default)
-            vi_sweep_dense_kernel<<<(unsigned)((n_rows + 127) / 128), 128, 0, stream>>>(g);
-        else
-            vi_sweep_dense_group_kernel<<<(unsigned)((n_rows + 31) / 32), 256, 0, stream>>>(g);
+        vi_sweep_dense_group_kernel<<<(unsigned)((n_rows + 31) / 32), 256, 0, stream>>>(g);
         vi_rowmax_kernel<<<(unsigned)((g.rows + 255) / 256), 256, 0, stream>>>(g);
         B2_CUDA_CHECK(cudaGetLastError());
         return B2_OK;
@@ -526,7 +368,7 @@ extern "C" int b2_vi_sweep(const b2_vi_problem* p, const double* v_in, const dou
     const int E = g.A * g.B;
     B2_REQUIRE(E <= 8192, "n_actions * n_next > 8192 not supported by the tiled kernel");
     // register kernel: B in {1,2,4,8}, A a power of two <= 32, vector-load alignment
-    if (p->reserved == 0 && (g.A & (g.A - 1)) == 0 && g.A <= 32 && (g.B == 1 || g.B == 2 || g.B == 4 || g.B == 8) &&
+    if ((g.A & (g.A - 1)) == 0 && g.A <= 32 && (g.B == 1 || g.B == 2 || g.B == 4 || g.B == 8) &&
         (uintptr_t)g.N % 16 == 0 && (!g.P || (uintptr_t)g.P % 16 == 0)) {
         const int64_t n_sa = g.rows * g.A;
         const int64_t blocks = (n_sa + 255) / 256;
@@ -539,39 +381,6 @@ extern "C" int b2_vi_sweep(const b2_vi_problem* p, const double* v_in, const dou
 #undef B2_ROW
         B2_CUDA_CHECK(cudaGetLastError());
         return B2_OK;
-    }
-    {
-        // TMA-staged kernel: tiles of TS states (TS % 16 == 0 keeps every bulk copy 16-byte sized/aligned;
-        // the last, ragged tile must still satisfy that, else fall back to the plain kernel)
-        int ts = (4096 / E) & ~15;
-        if (ts > 256) ts = 256;
-        const int64_t tail = g.rows % (ts > 0 ? ts : 1);
-        const bool tail_ok = (tail * E * 4) % 16 == 0 && (tail * g.A * 8) % 16 == 0 && tail % 16 == 0;
-        const bool aligned = ((uintptr_t)g.N % 16 == 0) && ((uintptr_t)g.R % 16 == 0) && ((uintptr_t)g.q_old % 16 == 0) &&
-                             ((uintptr_t)g.term % 16 == 0) && (!g.P || (uintptr_t)g.P % 16 == 0);
-        // p->reserved: 0 auto, 1 force the plain kernel, 2 force the TMA-staged kernel
-        const bool want_tma = p->reserved == 2;   // measured: never faster than the plain kernel (DESIGN.md 4.3)
-        if (want_tma && ts >= 16 && tail_ok && aligned) {
-            TileLayout lay;
-            int off = 0;
-            lay.p = off; off += ts * E * 8;      // products (and the P tile in sparse mode)
-            lay.n = off; off += ts * E * 4;
-            lay.r = off; off += ts * g.A * 8;
-            lay.q = off; off += ts * g.A * 8;
-            lay.t = off; off += (ts + 15) & ~15;
-            lay.bytes = (off + 127) & ~127;
-            const size_t smem_tma = (size_t)TMA_STAGES * lay.bytes + (size_t)ts * g.A * 8;
-            if (smem_tma <= 220 * 1024) {
-                B2_CUDA_CHECK(cudaFuncSetAttribute(vi_sweep_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-                g.tile_states = ts;
-                const int64_t n_tiles = (g.rows + ts - 1) / ts;
-                const int64_t sms = sm_count();
-                const unsigned grid = (unsigned)(n_tiles < sms ? n_tiles : sms);
-                vi_sweep_tma_kernel<<<grid, TMA_THREADS, smem_tma, stream>>>(g, lay);
-                B2_CUDA_CHECK(cudaGetLastError());
-                return B2_OK;
-            }
-        }
     }
     int tile = 4096 / E;
     if (tile < 1) tile = 1;

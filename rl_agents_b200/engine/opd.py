@@ -43,7 +43,8 @@ class _OPDTrees(HostTieEngine):
 
 
 class OPDEngine(_OPDTrees):
-    """n_trees independent OPD decisions per launch (one CTA per tree)."""
+    """n_trees independent OPD decisions per launch (one CTA per tree).  `kernel` fills b2_opd_config.reserved,
+    which must be 0: plan() raises B2Error otherwise."""
 
     def __init__(self, env_kind, n_trees, n_actions, budget, gamma, terminal_reward=0.0, mdp=None,
                  device="cuda", keys_in_smem=False, kernel=0):

@@ -188,11 +188,12 @@ def test_vi_sparse_random_vs_oracle(S, A, B, seed):
 
 @pytest.mark.parametrize("mode,S,A,B,seed", [("sparse", 4096, 8, 4, 0), ("sparse", 1600, 8, 4, 1), ("sparse", 6400, 4, 2, 2),
                                              ("sparse", 2048, 3, 9, 3), ("deterministic", 2048, 4, 1, 4),
-                                             ("deterministic", 5120, 8, 1, 5), ("sparse", 3200, 8, 8, 6)])
-@pytest.mark.parametrize("kernel", [0, 1, 2])
-def test_vi_kernel_variants_vs_oracle(mode, S, A, B, seed, kernel):
-    """The three sweep kernels (0: register rows when the shape allows, 1: tiled, 2: TMA-staged
-    tiles with a ragged last tile) all stay bit-identical with numpy."""
+                                             ("deterministic", 5120, 8, 1, 5), ("sparse", 3200, 8, 8, 6),
+                                             ("deterministic", 3000, 3, 1, 7), ("sparse", 1000, 4, 3, 8)])
+def test_vi_kernel_variants_vs_oracle(mode, S, A, B, seed):
+    """Both sweep kernels stay bit-identical with numpy.  A a power of two <= 32 with B in {1, 2, 4, 8} takes the
+    register kernel (vi_sweep_row_kernel); every other shape takes the tiled gather kernel (vi_sweep_gather_kernel),
+    here A = 3 in both modes and A = 4 with B = 3, each with a ragged last tile."""
     from rl_agents_b200.engine.vi import VIEngine
     term = np.random.default_rng(seed).uniform(size=S) < 0.03
     if mode == "sparse":
@@ -203,17 +204,15 @@ def test_vi_kernel_variants_vs_oracle(mode, S, A, B, seed, kernel):
         T, R = oenvs.garnet(S, A, 1, seed=seed, deterministic=True)
         q_ref, sweeps_ref = planners.value_iteration("deterministic", T, R, term, 0.9, 25)
         eng = VIEngine("deterministic", T, R, term, gamma=0.9)
-    eng.problem.reserved = kernel
     q, sweeps = eng.solve(25)
     assert sweeps == sweeps_ref
     assert np.array_equal(q.cpu().numpy(), q_ref)
 
 
 @pytest.mark.parametrize("S,A,seed", [(100, 4, 0), (5, 2, 1), (129, 3, 2), (300, 2, 3), (1000, 4, 4), (2051, 1, 5)])
-@pytest.mark.parametrize("kernel", [0, 1])
-def test_vi_dense_kernels_follow_numpy_pairwise_order(S, A, seed, kernel):
-    """Dense (stochastic) mode: the 8-lanes-per-row kernel (default) and the thread-per-row kernel both
-    reproduce numpy's pairwise summation bit for bit -- < 8, <= 128 and recursive-halving row lengths."""
+def test_vi_dense_kernels_follow_numpy_pairwise_order(S, A, seed):
+    """Dense (stochastic) mode: the 8-lanes-per-row kernel reproduces numpy's pairwise summation bit for bit --
+    < 8, <= 128 and recursive-halving row lengths."""
     from rl_agents_b200.engine.vi import VIEngine
     rng = np.random.default_rng(seed)
     P = rng.uniform(size=(S, A, S))
@@ -222,7 +221,6 @@ def test_vi_dense_kernels_follow_numpy_pairwise_order(S, A, seed, kernel):
     term = rng.uniform(size=S) < 0.05
     q_ref, sweeps_ref = planners.value_iteration("stochastic", P, R, term, 0.9, 12)
     eng = VIEngine("stochastic", P, R, term, gamma=0.9)
-    eng.problem.reserved = kernel
     q, sweeps = eng.solve(12)
     assert sweeps == sweeps_ref
     assert np.array_equal(q.cpu().numpy(), q_ref)
@@ -360,11 +358,11 @@ def test_opd_large_budget_invariants():
     assert pa == pb and torch.equal(a.upper, b.upper) and torch.equal(a.count, b.count) and torch.equal(a.parent, b.parent)
 
 
-def run_opd_highway(words_list, budget, gamma, keys_in_smem=False, kernel=0):
+def run_opd_highway(words_list, budget, gamma, keys_in_smem=False):
     import torch
     from rl_agents_b200 import _lib
     from rl_agents_b200.engine.opd import OPDEngine
-    eng = OPDEngine(_lib.ENV_HIGHWAY, len(words_list), 5, budget, gamma, keys_in_smem=keys_in_smem, kernel=kernel)
+    eng = OPDEngine(_lib.ENV_HIGHWAY, len(words_list), 5, budget, gamma, keys_in_smem=keys_in_smem)
     eng.plan(torch.tensor(np.stack(words_list), dtype=torch.int32, device="cuda"))
     plans, res = eng.finish([np_random(0) for _ in words_list])
     return eng, plans, res
@@ -392,14 +390,12 @@ def test_opd_highway_batch_vs_oracle():
         assert np.array_equal(d["lower"], np.array(t.lower)) and np.array_equal(d["upper"], np.array(t.upper))
 
 
-@pytest.mark.parametrize("kernel", [0, 1, 2])
-def test_opd_highway_packed_batch_equals_single_tree_search(kernel):
-    """>= 16 trees take a batch kernel (0: 8 trees per CTA, children of different trees share the
-    simulation slots, block barriers between the phases; 1: one tree per warp; 2: 8 trees per CTA as a dataflow over
-    a shared work ring, no block barriers); every tree must equal the one-tree-per-CTA search and the oracle."""
+def test_opd_highway_packed_batch_equals_single_tree_search():
+    """>= 16 trees take the batch kernel (8 trees per CTA, children of different trees share the simulation slots,
+    block barriers between the phases); every tree must equal the one-tree-per-CTA search and the oracle."""
     seeds = list(range(40, 59))          # 19 trees: full CTAs + a partial one
     words = [oenvs.make_highway_state(s).pack() for s in seeds]
-    eng, plans, res = run_opd_highway(words, 150, 0.8, kernel=kernel)
+    eng, plans, res = run_opd_highway(words, 150, 0.8)
     for i in (0, 7, 8, 18):
         one, plans1, res1 = run_opd_highway([words[i]], 150, 0.8)
         a, b = eng.tree_dict(i), one.tree_dict(0)
@@ -592,6 +588,7 @@ def test_edge_cases_small_budgets_and_argument_validation():
     from rl_agents_b200 import _lib
     from rl_agents_b200.engine.mcts import MCTSEngine, pcg64_words
     from rl_agents_b200.engine.opd import OPDEngine
+    from rl_agents_b200.engine.vi import VIEngine
     # budget < action_space.n: zero expansions, empty plan (the reference's get_plan returns [] too)
     eng, plans, res = run_opd_finite(product_mdp(), 3, 0.9, [0, 1, 2])
     assert plans == [[], [], []] and res[:, 0].tolist() == [1, 1, 1] and eng.tree_dict(0)["count"].tolist() == [1]
@@ -617,17 +614,25 @@ def test_edge_cases_small_budgets_and_argument_validation():
     m.cfg.rollout_policy = 7
     with pytest.raises(_lib.B2Error, match="policy"):
         m.plan(torch.zeros(1, dtype=torch.int32, device="cuda"), pcg64_words(np_random(0)).reshape(1, -1))
+    # the reserved fields select nothing: any value but 0 is refused, not run as the default
+    for value in (1, 2):
+        hw = OPDEngine(_lib.ENV_HIGHWAY, 24, 5, 300, 0.8, kernel=value)
+        with pytest.raises(_lib.B2Error, match="reserved"):
+            hw.plan(torch.zeros(24, _lib.HW_STATE_WORDS, dtype=torch.int32, device="cuda"))
+        T, R = oenvs.garnet(64, 4, 1, seed=0, deterministic=True)
+        vi = VIEngine("deterministic", T, R, np.zeros(64, bool), gamma=0.9)
+        vi.problem.reserved = value
+        with pytest.raises(_lib.B2Error, match="reserved"):
+            vi.solve(3)
 
 
-@pytest.mark.parametrize("kernel", [0, 2])
-def test_opd_highway_c2_full_size_batch_vs_c_oracle(kernel):
-    """C2 at full size, many decisions: 24 scenes x budget 10 000 through the batch kernels (barrier and dataflow
-    variants), every node array of every tree bit-identical with the C oracle (itself pinned to the reference's
-    golden tree)."""
+def test_opd_highway_c2_full_size_batch_vs_c_oracle():
+    """C2 at full size, many decisions: 24 scenes x budget 10 000 through the batch kernel, every node array of every
+    tree bit-identical with the C oracle (itself pinned to the reference's golden tree)."""
     from oracle import c_oracle
     seeds = list(range(500, 524))
     words = [oenvs.make_highway_state(s).pack() for s in seeds]
-    eng, plans, res = run_opd_highway(words, 10000, 0.8, kernel=kernel)
+    eng, plans, res = run_opd_highway(words, 10000, 0.8)
     for i, w in enumerate(words):
         t = c_oracle.opd_plan(w, 10000, 0.8)
         d = eng.tree_dict(i)
