@@ -717,6 +717,67 @@ typedef struct b2_mcts_dpw_tree {
 int b2_mcts_dpw_plan(const b2_mcts_dpw_config* cfg, const int32_t* root_states, const b2_mcts_dpw_tree* tree,
                      uint64_t* rng, int8_t* plan, int32_t* result, void* stream);
 
+/* ------------------------------------------------------------------------
+ * PlaTyPOOS -- rl_agents/agents/tree_search/platypoos.py (PlaTyPOOS, PlaTyPOOSNode).  Finite MDPs in all three modes
+ * and HighwayLite.  The search runs one depth layer at a time; every table that needs log2, ceil, floor or pow comes
+ * from the host, evaluated with the reference's own expressions, so every node equals the reference's bit for bit.
+ * ---------------------------------------------------------------------- */
+typedef struct b2_platypoos_config {
+    int32_t env_kind;        /* B2_ENV_FINITE or B2_ENV_HIGHWAY                                                 */
+    int32_t n_trees;
+    int32_t n_actions;       /* finite: action_space.n, whose actions 1..n-1 are expanded (the reference's fallback
+                                range(1, n), :145-147); HighwayLite: 5, its available actions in env order      */
+    int32_t horizon;         /* h_max >= 2 (config["horizon"]): the root is expanded h_max times per action      */
+    int32_t node_capacity;   /* per tree; running out sets error 1                                              */
+    int32_t layer_capacity;  /* the widest depth layer per tree (scene, sort and selection slots); error 1 past it  */
+    int32_t max_p;           /* entries per depth in the quota tables: p_top(h) < max_p <= 32                    */
+    int32_t env_draws;       /* finite: 1 when the MDP is not "deterministic" (a new child's state is drawn by
+                                Generator.choice of the env copy seeded with its first sample's randint(2**30))   */
+    const int32_t* p_top;        /* [horizon] p_top(h) of explore(h) (:41), entry 0 unused                      */
+    const int32_t* nodes_count;  /* [horizon, max_p] at h * max_p + p (:44)                                      */
+    const int32_t* evaluations;  /* [horizon, max_p] (:45)                                                       */
+    const int32_t* min_visits;   /* [horizon, max_p] (:46)                                                       */
+    const int32_t* cv_count;     /* [horizon] cross_validate's evaluations at a node of depth d (:75-76)          */
+    const double* gamma_pow;     /* [horizon] gamma**d: a child of depth d + 1 has value parent.value + gamma**d *
+                                    cumulative_reward / count (:129-130)                                         */
+    const uint8_t* terminal;     /* finite: [S], `done` of a step taken in s                                      */
+    b2_finite_mdp_sampled mdp;   /* env_kind == FINITE                                                          */
+} b2_platypoos_config;
+
+/* The arena, [n_trees, node_capacity] per field; node id = creation order.  A node's children are contiguous, in its
+ * available-action order, from first_child. */
+typedef struct b2_platypoos_tree {
+    int32_t* parent;         /* -1 for the root                                                                  */
+    int32_t* first_child;    /* -1 until the node is expanded with at least one sample                           */
+    int32_t* action;         /* the incoming action, -1 at the root                                              */
+    int32_t* depth;
+    int32_t* count;          /* samples of the node's (parent state, action) (:127)                              */
+    int32_t* flags;          /* bit 0 done, bit 1 to_expand                                                       */
+    int32_t* state;          /* finite: the state id the first sample reached; HighwayLite: its available-action
+                                mask                                                                             */
+    double* cumulative;      /* cumulative_reward (:126)                                                          */
+    double* value;           /* value (:128-129); the root's is 0.0                                               */
+    double* reward;          /* the reward of the node's (parent state, action) step                             */
+} b2_platypoos_tree;
+
+#define B2_PLATYPOOS_RESULT_WORDS 8
+/* per tree int32 result: [0] nodes [1] openings (the reference logs them, :95) [2] plan length [3] error (1: node or
+ * layer capacity exhausted; 2: a sampled probability row that Generator.choice rejects, reached; 3: cross-validation
+ * would create a child; 4: no candidate) [4] the rejected row, s * n_actions + a (-1 otherwise) [5] env steps (one per
+ * created child) [6] candidates [7] 0 */
+
+/* Bytes of scratch per call: per tree the two ping-pong layers of HighwayLite scenes and the sort and selection lists
+ * of one layer. */
+int64_t b2_platypoos_workspace_bytes(const b2_platypoos_config* cfg);
+
+/* PlaTyPOOS.plan (:88-97) for n_trees independent decisions, one tree per CTA.  rng: uint64 [n_trees, 6] numpy PCG64
+ * states of the planners' streams, advanced in place by every randint(2**30) the reference draws; root_states:
+ * [n_trees] state ids or [n_trees, 136] words; plan: int8 [n_trees, horizon], the actions from the root to the best
+ * candidate (result word 2 of them); candidates: int32 [n_trees, 2 * max_p], (p, node id) pairs in dict order. */
+int b2_platypoos_plan(const b2_platypoos_config* cfg, const int32_t* root_states, const b2_platypoos_tree* tree,
+                      void* workspace, uint64_t* rng, int8_t* plan, int32_t* candidates, int32_t* result,
+                      void* stream);
+
 #ifdef __cplusplus
 }
 #endif

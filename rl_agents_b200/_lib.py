@@ -23,6 +23,7 @@ MDP_GAPE_RESULT_WORDS = 8
 BRUE_RESULT_WORDS = 8
 SPARSE_SAMPLING_RESULT_WORDS = 8
 MCTS_DPW_RESULT_WORDS = 8
+PLATYPOOS_RESULT_WORDS = 8
 PCG64_STATE_WORDS = 6
 
 
@@ -197,6 +198,21 @@ class MCTSDPWTree(ctypes.Structure):
     _fields_ = [(n, c_void_p) for n in MCTS_DPW_TREE_FIELDS]
 
 
+class PlaTyPOOSConfig(ctypes.Structure):
+    _fields_ = [("env_kind", c_int32), ("n_trees", c_int32), ("n_actions", c_int32), ("horizon", c_int32),
+                ("node_capacity", c_int32), ("layer_capacity", c_int32), ("max_p", c_int32), ("env_draws", c_int32),
+                ("p_top", c_void_p), ("nodes_count", c_void_p), ("evaluations", c_void_p), ("min_visits", c_void_p),
+                ("cv_count", c_void_p), ("gamma_pow", c_void_p), ("terminal", c_void_p), ("mdp", FiniteMDPSampled)]
+
+
+PLATYPOOS_TREE_FIELDS = ("parent", "first_child", "action", "depth", "count", "flags", "state", "cumulative", "value",
+                         "reward")
+
+
+class PlaTyPOOSTree(ctypes.Structure):
+    _fields_ = [(n, c_void_p) for n in PLATYPOOS_TREE_FIELDS]
+
+
 EXPORTS = {
     "b2_last_error": (ctypes.c_char_p, []),
     "b2_version": (c_int, []),
@@ -255,6 +271,9 @@ EXPORTS = {
                                                ctypes.POINTER(SparseSamplingTree)] + [c_void_p] * 6),
     "b2_mcts_dpw_plan": (c_int, [ctypes.POINTER(MCTSDPWConfig), c_void_p, ctypes.POINTER(MCTSDPWTree), c_void_p,
                                  c_void_p, c_void_p, c_void_p]),
+    "b2_platypoos_workspace_bytes": (c_int64, [ctypes.POINTER(PlaTyPOOSConfig)]),
+    "b2_platypoos_plan": (c_int, [ctypes.POINTER(PlaTyPOOSConfig), c_void_p, ctypes.POINTER(PlaTyPOOSTree)]
+                          + [c_void_p] * 6),
 }
 
 _lib = None

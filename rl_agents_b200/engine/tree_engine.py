@@ -10,7 +10,8 @@ from rl_agents_b200 import _lib
 from rl_agents_b200.engine.tables import gamma_tables, terminal_bonus_table
 
 # node fields stored as int32; every other node field is float64
-INT32_FIELDS = ("parent", "first_child", "next_sibling", "count", "meta", "kind", "key", "depth", "obs")
+INT32_FIELDS = ("parent", "first_child", "next_sibling", "count", "meta", "kind", "key", "depth", "obs", "action",
+                "flags", "state")
 
 
 def decode_action(meta):

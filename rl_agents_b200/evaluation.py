@@ -17,8 +17,9 @@ def _np_random(seed):
 def run_batched_episodes(planner, seeds, budget, gamma, max_steps=40, device="cuda", planner_seed=0, **kw):
     """planner: "opd" | "mcts" | "olop" | "mdp_gape" (keywords: MDPGapEAgent config keys) | "brue" (keywords: BRUEAgent
     config keys) | "sparse_sampling" (keywords `horizon` and `C`, required as in SparseSamplingAgent's config; `budget`
-    is unused) | "mcts_dpw" (keywords: MCTSDPWAgent config keys) | "vi" (ValueIterationAgent on the scenes' TTC-grid
-    MDPs, `budget` = its `iterations`).  Every episode: scene make_scene(seed), replanning at every step (receding_horizon 1, step_strategy reset -- the reference
+    is unused) | "mcts_dpw" (keywords: MCTSDPWAgent config keys) | "platypoos" (keywords: PlaTyPOOSAgent config keys;
+    the first action of each plan is played) | "vi" (ValueIterationAgent on the scenes' TTC-grid MDPs, `budget` = its
+    `iterations`).  Every episode: scene make_scene(seed), replanning at every step (receding_horizon 1, step_strategy reset -- the reference
     defaults), until crash or `max_steps`.
     Returns dict(returns, lengths, crashed, decision_ms)."""
     import torch
@@ -77,6 +78,14 @@ def run_batched_episodes(planner, seeds, budget, gamma, max_steps=40, device="cu
                             pcfg["alpha_action"], pcfg["k_state"], pcfg["alpha_state"],
                             closed_loop=pcfg["closed_loop"],
                             rollout_policy=MCTSDPWAgent.policy_factory(pcfg["rollout_policy"]), device=dev)
+    elif planner == "platypoos":
+        # PlaTyPOOSAgent's completed planner config (h_max from the budget unless "horizon" is given)
+        from rl_agents_b200.agents.tree_search.platypoos import PlaTyPOOS
+        from rl_agents_b200.engine.platypoos import PlaTyPOOSEngine, horizon_of
+        cfg = PlaTyPOOS.default_config()
+        PlaTyPOOS.rec_update(cfg, dict(kw, budget=budget, gamma=gamma))
+        horizon = cfg["horizon"] if "horizon" in cfg else horizon_of(budget, 5)
+        eng = PlaTyPOOSEngine(_lib.ENV_HIGHWAY, n, 5, horizon, gamma, device=dev)
     elif planner == "vi":
         from rl_agents_b200.engine.ttc_vi import HighwayTTCVI
         eng = HighwayTTCVI(gamma, budget, device=dev)
