@@ -38,7 +38,7 @@ int b2_device_info(int* sm_count, int* cc_major, int* cc_minor, char* name, int 
 #define B2_ENV_FINITE 0   /* finite MDP tables (deterministic, except for sparse sampling) */
 #define B2_ENV_HIGHWAY 1  /* HighwayLite, docs/HIGHWAY_LITE_SPEC.md         */
 
-#define B2_ENV_INTERSECTION 2 /* IntersectionLite, docs/INTERSECTION_LITE_SPEC.md (wavefront OPD + b2_intersection_step) */
+#define B2_ENV_INTERSECTION 2 /* IntersectionLite, docs/INTERSECTION_LITE_SPEC.md (wavefront OPD, MCTS, OLOP + b2_intersection_step) */
 
 #define B2_HW_STATE_WORDS 136 /* 32-bit words of one HighwayLite / IntersectionLite state */
 #define B2_HW_ACTIONS 5
@@ -413,7 +413,8 @@ typedef struct b2_mcts_tree {
 /* MCTS.plan (:179-184) for n_trees independent decisions, strict episode order
  * inside each tree, consuming each tree's numpy PCG64 stream exactly as
  * Generator.choice does (abstract.py:304-311, mcts.py:172).  rng: uint64
- * [n_trees, 6] numpy bit-generator states, advanced in place.  plan: int8 [n_trees, horizon]. */
+ * [n_trees, 6] numpy bit-generator states, advanced in place.  plan: int8 [n_trees, horizon].
+ * env_kind: B2_ENV_FINITE, B2_ENV_HIGHWAY (5 actions) or B2_ENV_INTERSECTION (3 actions). */
 int b2_mcts_plan(const b2_mcts_config* cfg, const int32_t* root_states, const b2_mcts_tree* tree,
                  uint64_t* rng, int8_t* plan, int32_t* result, void* stream);
 
@@ -489,7 +490,7 @@ typedef struct b2_olop_tree {
  * [2] error (1: reward outside [0,1], olop.py:133-134; 2: "zeros" continuation
  *     with action 0 unavailable -- a KeyError in the reference, :82,:88) */
 
-/* OLOP.plan (:94-100); rng as in b2_mcts_plan; plan: int8 [n_trees, horizon]. */
+/* OLOP.plan (:94-100); rng and env_kind as in b2_mcts_plan; plan: int8 [n_trees, horizon]. */
 int b2_olop_plan(const b2_olop_config* cfg, const int32_t* root_states, const b2_olop_tree* tree,
                  uint64_t* rng, int8_t* plan, int32_t* result, void* stream);
 

@@ -32,8 +32,8 @@ class MCTS(AbstractPlanner):
         self.rollout_policy = rollout_policy
         if not self.config["horizon"]:                                   # mcts.py:116-118
             self.config["episodes"], self.config["horizon"] = allocation(self.config["budget"], self.config["gamma"])
-        # closed_loop (mcts.py:125,147,267-273) keys an extra node level on str(observation).  Both device env
-        # models are deterministic: every action node then has exactly one observation child carrying the same
+        # closed_loop (mcts.py:125,147,267-273) keys an extra node level on str(observation).  The device env
+        # models (finite MDPs, HighwayLite, IntersectionLite) are deterministic: every action node then has exactly one observation child carrying the same
         # statistics, so visit counts, values and the recommended action equal the open-loop search's
         # (golden: tests/golden "mcts_closed_loop", produced by the reference with closed_loop=True).  The
         # reference's get_plan interleaves the observation keys with the actions; here the plan lists actions.

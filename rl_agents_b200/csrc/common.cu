@@ -35,6 +35,14 @@ int check_lane_env(int env_kind, int n_actions, const b2_finite_mdp& mdp) {
     }
     return check_env_kind(env_kind, n_actions);
 }
+
+int check_lane_env_il(int env_kind, int n_actions, const b2_finite_mdp& mdp) {
+    if (env_kind == B2_ENV_INTERSECTION) {
+        B2_REQUIRE(n_actions == B2_IL_ACTIONS, "IntersectionLite has 3 actions");
+        return B2_OK;
+    }
+    return check_lane_env(env_kind, n_actions, mdp);
+}
 }  // namespace b2
 
 extern "C" const char* b2_last_error(void) { return b2::g_err; }

@@ -32,9 +32,11 @@ int sm_count();
 
 // Launch checks of the planners that run one tree per lane group.  Both return B2_OK, or B2_ERR_INVALID with the
 // error set.  check_env_kind: a known env_kind, and HighwayLite's 5 actions; check_lane_env also requires the
-// finite tables and their action count.
+// finite tables and their action count.  check_lane_env_il (MCTS and OLOP, the planners with an IntersectionLite
+// model) also accepts IntersectionLite with its 3 actions; the other planners keep refusing it.
 int check_env_kind(int env_kind, int n_actions);
 int check_lane_env(int env_kind, int n_actions, const b2_finite_mdp& mdp);
+int check_lane_env_il(int env_kind, int n_actions, const b2_finite_mdp& mdp);
 
 // Blocks of 128 threads for n_trees trees of `group` lanes each.
 inline int lane_grid(int n_trees, int group) { return (n_trees * group + 127) / 128; }

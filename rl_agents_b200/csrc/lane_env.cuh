@@ -1,7 +1,7 @@
 // Device env models of the one-tree-per-lane-group planners (mcts.cu, olop.cu, mdp_gape.cu, brue.cu): one tree per
-// lane on a finite MDP, one tree per 16-lane group on HighwayLite (lane = vehicle slot, the scene in registers, so
-// the reference's deep copy of the env is a register copy).  Each model reads only what it needs: the finite tables,
-// the root states and the action count.
+// lane on a finite MDP, one tree per 16-lane group on HighwayLite and IntersectionLite (lane = vehicle slot, the scene
+// in registers, so the reference's deep copy of the env is a register copy).  Each model reads only what it needs: the
+// finite tables, the root states and the action count.
 //
 // step() reports truncation separately; MCTS reads it, the other planners pass a dummy (the reference's 4-tuple step
 // drops truncation).
@@ -11,6 +11,7 @@
 #pragma once
 #include "common.cuh"
 #include "highway_lite.cuh"
+#include "intersection_lite.cuh"
 #include "pcg64.cuh"
 
 namespace b2 {
@@ -78,6 +79,34 @@ struct HighwayEnv {
     __device__ __forceinline__ double step(const b2_finite_mdp& m, int action, int li, unsigned gmask,
                                            bool& term, bool& trunc) {
         return (double)hw::step(L, li, t, si, action, term, trunc, gmask);
+    }
+};
+
+// IntersectionLite (mcts.cu and olop.cu only): the same 16-lane group and 136-word slot as HighwayLite; three actions
+// offered in the env's order IDLE, FASTER, SLOWER, which is not ascending action id.
+struct IntersectionEnv {
+    static constexpr int GROUP = 16;
+    il::Lane L;
+    il::Globals g;
+    __device__ __forceinline__ void load_root(const int32_t* root_states, int tree, int li) {
+        il::load_state<false>(root_states + (int64_t)tree * il::WORDS, li, L, g);
+    }
+    __device__ __forceinline__ int avail(int n_actions, unsigned gmask) const { return il::avail_mask(g.si); }
+    __device__ __forceinline__ static int nth(int mask, int n) { return il::nth_action(mask, n); }
+    __device__ __forceinline__ static int rank_of(int mask, int action) {
+        if (action < 0 || !((mask >> action) & 1)) return -1;
+        const int order[3] = {il::A_IDLE, il::A_FASTER, il::A_SLOWER};
+        int k = 0;
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+            if (order[i] == action) return k;
+            k += (mask >> order[i]) & 1;
+        }
+        return -1;
+    }
+    __device__ __forceinline__ double step(const b2_finite_mdp& m, int action, int li, unsigned gmask,
+                                           bool& term, bool& trunc) {
+        return (double)il::step(L, li, g, action, term, trunc, gmask);
     }
 };
 

@@ -5,7 +5,7 @@
 // tree indices, visit counts and values are bit-identical; the batch dimension
 // (thousands of trees / root-parallel replicas) is what fills the GPU.
 //
-// One tree per lane group: 16 lanes for HighwayLite (lane = vehicle slot, the
+// One tree per lane group: 16 lanes for HighwayLite and IntersectionLite (lane = vehicle slot, the
 // scene lives in registers and is "deep-copied" from the root once per episode,
 // mcts.py:183), 1 lane for finite MDPs.  Tree bookkeeping is group-uniform
 // scalar code; lane 0 of the group performs the stores.
@@ -64,6 +64,8 @@ __global__ void __launch_bounds__(128, B2_MCTS_MIN_BLOCKS) mcts_kernel(MctsArgs 
             // the 16 lanes of a group leave the episode together (terminal / truncated); the
             // other half of the warp keeps stepping its own scene under its half mask
             if (!active) break;
+            // what a group that left its episode steps (the result is dropped): IDLE, action 1 on HighwayLite and
+            // IntersectionLite alike (il::A_IDLE == hw::A_IDLE), always available there
             int action = hw::A_IDLE < A ? hw::A_IDLE : 0, child = -1;
             const int amask = env.avail(a.cfg.n_actions, gmask);
             if (active && in_sel && tr.first_child[nb + node] < 0) {
@@ -200,15 +202,17 @@ extern "C" int b2_mcts_plan(const b2_mcts_config* cfg, const int32_t* root_state
                "policy must be 0 (random_available), 1 (random) or 2 (preference)");
     B2_REQUIRE((cfg->prior_policy != 2 || cfg->pref_prior) && (cfg->rollout_policy != 2 || cfg->pref_cdf),
                "preference policy tables missing");
-    const int rc = check_lane_env(cfg->env_kind, cfg->n_actions, cfg->mdp);
+    const int rc = check_lane_env_il(cfg->env_kind, cfg->n_actions, cfg->mdp);
     if (rc != B2_OK) return rc;
     cudaStream_t stream = (cudaStream_t)stream_;
     MctsArgs a;
     a.cfg = *cfg; a.tree = *tree; a.root_states = root_states; a.rng = rng; a.plan = plan; a.result = result;
     if (cfg->env_kind == B2_ENV_FINITE)
         mcts_kernel<FiniteEnv><<<lane_grid(cfg->n_trees, FiniteEnv::GROUP), 128, 0, stream>>>(a);
-    else
+    else if (cfg->env_kind == B2_ENV_HIGHWAY)
         mcts_kernel<HighwayEnv><<<lane_grid(cfg->n_trees, HighwayEnv::GROUP), 128, 0, stream>>>(a);
+    else
+        mcts_kernel<IntersectionEnv><<<lane_grid(cfg->n_trees, IntersectionEnv::GROUP), 128, 0, stream>>>(a);
     B2_CUDA_CHECK(cudaGetLastError());
     return B2_OK;
 }

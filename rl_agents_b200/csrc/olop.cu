@@ -6,8 +6,8 @@
 // (rl_agents/utils.py:123-203: damped Newton iteration on the Bernoulli KL,
 // kl_bound.cuh) runs in-kernel in fp64.
 //
-// Same lane-group mapping as mcts.cu: one tree per 16-lane group (HighwayLite,
-// lane = vehicle slot) or per lane (finite MDP).
+// Same lane-group mapping as mcts.cu: one tree per 16-lane group (HighwayLite and
+// IntersectionLite, lane = vehicle slot) or per lane (finite MDP).
 #include "common.cuh"
 #include "kl_bound.cuh"
 #include "lane_env.cuh"
@@ -174,15 +174,17 @@ extern "C" int b2_olop_plan(const b2_olop_config* cfg, const int32_t* root_state
     B2_REQUIRE((int64_t)cfg->node_capacity >= 1 + (int64_t)cfg->episodes * cfg->horizon * cfg->n_actions,
                "node_capacity too small");
     B2_REQUIRE(cfg->thresholds && cfg->init_upper, "threshold / initial bound tables missing");
-    const int rc = check_lane_env(cfg->env_kind, cfg->n_actions, cfg->mdp);
+    const int rc = check_lane_env_il(cfg->env_kind, cfg->n_actions, cfg->mdp);
     if (rc != B2_OK) return rc;
     cudaStream_t stream = (cudaStream_t)stream_;
     OlopArgs a;
     a.cfg = *cfg; a.tree = *tree; a.root_states = root_states; a.rng = rng; a.plan = plan; a.result = result;
     if (cfg->env_kind == B2_ENV_FINITE)
         olop_kernel<FiniteEnv><<<lane_grid(cfg->n_trees, FiniteEnv::GROUP), 128, 0, stream>>>(a);
-    else
+    else if (cfg->env_kind == B2_ENV_HIGHWAY)
         olop_kernel<HighwayEnv><<<lane_grid(cfg->n_trees, HighwayEnv::GROUP), 128, 0, stream>>>(a);
+    else
+        olop_kernel<IntersectionEnv><<<lane_grid(cfg->n_trees, IntersectionEnv::GROUP), 128, 0, stream>>>(a);
     B2_CUDA_CHECK(cudaGetLastError());
     return B2_OK;
 }

@@ -1,5 +1,5 @@
-"""Batched closed-loop evaluation of the planners on HighwayLite: the working version of the
-reference's disabled budget-sweep harness (scripts/planners_evaluation.py:287-289, SURVEY 8f
+"""Batched closed-loop evaluation of the planners on HighwayLite (and of MCTS and OLOP on IntersectionLite): the
+working version of the reference's disabled budget-sweep harness (scripts/planners_evaluation.py:287-289, SURVEY 8f
 rank 4) in the shape the GPU wants -- all episodes advance in lock-step, every decision step is
 ONE batched plan() launch over all live episodes and ONE batched env transition."""
 import time
@@ -7,26 +7,42 @@ import time
 import numpy as np
 
 from rl_agents_b200 import _lib
-from rl_agents_b200.envs.highway_lite import make_scene
+from rl_agents_b200.envs import highway_lite, intersection_lite
+
+# planners with an IntersectionLite model (b2_mcts_plan, b2_olop_plan)
+INTERSECTION_PLANNERS = ("mcts", "olop")
 
 
 def _np_random(seed):
     return np.random.Generator(np.random.PCG64(np.random.SeedSequence(seed)))
 
 
-def run_batched_episodes(planner, seeds, budget, gamma, max_steps=40, device="cuda", planner_seed=0, **kw):
+def run_batched_episodes(planner, seeds, budget, gamma, max_steps=40, device="cuda", planner_seed=0, env="highway",
+                         **kw):
     """planner: "opd" | "mcts" | "olop" | "mdp_gape" (keywords: MDPGapEAgent config keys) | "brue" (keywords: BRUEAgent
     config keys) | "sparse_sampling" (keywords `horizon` and `C`, required as in SparseSamplingAgent's config; `budget`
     is unused) | "mcts_dpw" (keywords: MCTSDPWAgent config keys) | "platypoos" (keywords: PlaTyPOOSAgent config keys;
     the first action of each plan is played) | "vi" (ValueIterationAgent on the scenes' TTC-grid MDPs, `budget` = its
     `iterations`).  Every episode: scene make_scene(seed), replanning at every step (receding_horizon 1, step_strategy reset -- the reference
     defaults), until crash or `max_steps`.
+    env: "highway" (HighwayLite, every planner) or "intersection" (IntersectionLite scenes of
+    envs.intersection_lite.make_scene stepped by b2_intersection_step, "mcts" and "olop" only; an episode also ends
+    when the ego arrives or at the env's duration).  `crashed` is the ego's crash flag.
     Returns dict(returns, lengths, crashed, decision_ms)."""
     import torch
     from rl_agents_b200.engine.mcts import MCTSEngine, pcg64_words, set_pcg64_words
     from rl_agents_b200.engine.olop import OLOPEngine
     from rl_agents_b200.engine.opd import OPDEngine
     from rl_agents_b200.agents.tree_search.mcts import allocation
+    if env == "highway":
+        env_kind, n_actions, make_scene = _lib.ENV_HIGHWAY, 5, highway_lite.make_scene
+    elif env == "intersection":
+        if planner not in INTERSECTION_PLANNERS:
+            raise NotImplementedError("%r runs on HighwayLite only; IntersectionLite runs %s"
+                                      % (planner, " and ".join(INTERSECTION_PLANNERS)))
+        env_kind, n_actions, make_scene = _lib.ENV_INTERSECTION, intersection_lite.N_ACTIONS, intersection_lite.make_scene
+    else:
+        raise ValueError("unknown env %r" % env)
     lib = _lib.load()
     dev = torch.device(device)
     n = len(seeds)
@@ -38,12 +54,12 @@ def run_batched_episodes(planner, seeds, budget, gamma, max_steps=40, device="cu
         episodes, horizon = allocation(budget, gamma)
         from rl_agents_b200.agents.tree_search.mcts import MCTS
         # the reference's default temperature comes from the CLASS default gamma (mcts.py:120-127), not the configured one
-        eng = MCTSEngine(_lib.ENV_HIGHWAY, n, 5, episodes, horizon, gamma,
+        eng = MCTSEngine(env_kind, n, n_actions, episodes, horizon, gamma,
                          kw.get("temperature", MCTS.default_config()["temperature"]), device=dev)
     elif planner == "olop":
-        episodes, horizon = allocation(max(5, budget), gamma)
+        episodes, horizon = allocation(max(n_actions, budget), gamma)
         ub = kw.get("upper_bound", {"type": "kullback-leibler", "time": "global", "threshold": "2*np.log(time)"})
-        eng = OLOPEngine(_lib.ENV_HIGHWAY, n, 5, episodes, horizon, gamma, ub, kw.get("continuation_type", "uniform"),
+        eng = OLOPEngine(env_kind, n, n_actions, episodes, horizon, gamma, ub, kw.get("continuation_type", "uniform"),
                          device=dev)
     elif planner == "mdp_gape":
         # MDPGapEAgent's completed config (mdp_gape.py:20-40) with budget / gamma and any keyword overriding it
@@ -116,13 +132,17 @@ def run_batched_episodes(planner, seeds, budget, gamma, max_steps=40, device="cu
         t_plan += time.perf_counter() - t0
         act = np.array([p[0] if p else 1 for p in plans], dtype=np.int32)      # empty plan: IDLE
         actions_log.append(act.copy())
-        _lib.check(lib.b2_highway_step(_lib.ptr(scenes), _lib.ptr(torch.from_numpy(act).to(dev)), _lib.ptr(rew),
-                                       _lib.ptr(flg), None, n, _lib.current_stream()))
+        step = lib.b2_highway_step if env == "highway" else lib.b2_intersection_step
+        _lib.check(step(_lib.ptr(scenes), _lib.ptr(torch.from_numpy(act).to(dev)), _lib.ptr(rew), _lib.ptr(flg), None, n,
+                        _lib.current_stream()))
         r, f = rew.cpu().numpy(), flg.cpu().numpy()
         returns += np.where(alive, r, 0.0)
         lengths += alive
         done = (f & 3) != 0
-        crashed |= alive & ((f & 1) != 0)
+        if env == "highway":
+            crashed |= alive & ((f & 1) != 0)
+        else:       # IntersectionLite also terminates on arrival: the crash is bit 1 of the ego's flags word
+            crashed |= alive & ((scenes[:, 48].cpu().numpy() & 2) != 0)
         alive &= ~done
     return {"returns": returns, "lengths": lengths, "crashed": crashed, "actions": np.array(actions_log).T,
             "decision_ms": 1e3 * t_plan / max(len(actions_log), 1), "n": n}
