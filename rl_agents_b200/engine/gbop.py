@@ -1,13 +1,33 @@
-"""Batched GBOP-T engine (device side of StateAwarePlannerAgent)."""
+"""Batched GBOP-T and GBOP-D engines (device side of StateAwarePlannerAgent and GraphBasedPlannerAgent).
+
+Both GBOP kernels keep their breadth-first backup queue as a linear array of `queue_capacity` entries per tree and
+report a backup that would push past it in result word 7.  How many entries one backup needs is not bounded by any
+fixed multiple of the tree or state count (it grows faster than the budget), so the engines recover: finish() doubles
+the queue, reallocates it and relaunches the same search until no tree overflows.  The kernels are deterministic,
+so the relaunched search is bit for bit the one a large enough queue would have run, and the grown size is kept for
+the engine's later searches.  A queue thus holds fewer than twice the entries of the largest backup the engine has
+run (or its first size), n_trees times over.  Only a queue that would need more than 2**31 - 1 entries (the kernels
+index it with int32) is an error."""
 import numpy as np
 
 from rl_agents_b200 import _lib
 from rl_agents_b200.engine.tables import FiniteTables
 from rl_agents_b200.engine.tree_engine import HostTieEngine, TreeEngine, decode_action
 
+QUEUE_CAPACITY_MAX = 2 ** 31 - 1
+
+
+def grown_queue_capacity(capacity, name):
+    """The next backup queue size after an overflow at `capacity` entries: double, up to int32 indexing."""
+    if capacity >= QUEUE_CAPACITY_MAX:
+        raise _lib.B2Error("%s backup queue overflow: one backup needs more than 2**31 - 1 queue entries, "
+                           "beyond the kernel's int32 queue indexing" % name)
+    return min(2 * capacity, QUEUE_CAPACITY_MAX)
+
 
 class GBOPEngine(HostTieEngine):
-    """n_trees independent GBOP-T decisions per launch (one warp per tree) on a deterministic finite MDP."""
+    """n_trees independent GBOP-T decisions per launch (one warp per tree) on a deterministic finite MDP.
+    queue_factor: the first backup queue size per tree, in multiples of the node capacity (grown on overflow)."""
     # StateAwarePlanner.plan runs get_plan() twice (state_aware.py:124, :130; the first inside super().plan()): a tie
     # consumes the planner RNG on both walks, the second is returned
     TIE_WALKS = 2
@@ -19,10 +39,21 @@ class GBOPEngine(HostTieEngine):
         self.tables = FiniteTables(mdp, self.device)
         self.n_states = self.tables.n_states
         self.cfg = _lib.GBOPConfig(self.n_trees, self.n_actions, self.n_expansions, self.capacity, self.plan_capacity,
-                                   int(queue_factor) * self.capacity, 1 if backup_aggregated_nodes else 0,
-                                   1 if prune_suboptimal_leaves else 0, gamma, 1 / (1 - gamma), accuracy * (1 - gamma),
-                                   self.gamma_pow.data_ptr(), self.terminal_bonus.data_ptr(), self.tables.struct())
+                                   min(int(queue_factor) * self.capacity, QUEUE_CAPACITY_MAX),
+                                   1 if backup_aggregated_nodes else 0, 1 if prune_suboptimal_leaves else 0, gamma,
+                                   1 / (1 - gamma), accuracy * (1 - gamma), self.gamma_pow.data_ptr(),
+                                   self.terminal_bonus.data_ptr(), self.tables.struct())
         self.tree = _lib.GBOPTree(*self._alloc_tree(_lib.GBOP_TREE_FIELDS, self.capacity))
+        self._alloc_workspace()
+        self.relaunches = 0          # searches run again after a queue overflow, over the engine's life
+        self._roots = None
+
+    @property
+    def queue_capacity(self):
+        return int(self.cfg.queue_capacity)
+
+    def _alloc_workspace(self):
+        """Per-tree workspace: state values, per-state node lists, expansion order, then the backup queue."""
         ws = self.lib.b2_gbop_workspace_bytes(self.cfg)
         if ws < 0:
             raise _lib.B2Error("unsupported GBOP configuration")
@@ -31,13 +62,20 @@ class GBOPEngine(HostTieEngine):
 
     def plan(self, root_states):
         assert root_states.dtype == self.torch.int32 and root_states.is_cuda and root_states.is_contiguous()
+        self._roots = root_states            # kept for a relaunch after a queue overflow
         _lib.check(self.lib.b2_gbop_plan(self.cfg, _lib.ptr(root_states), self.tree, _lib.ptr(self.workspace),
                                          _lib.ptr(self.plan_buf), _lib.ptr(self.result), _lib.current_stream()))
 
-    def _check(self, res):
-        super(GBOPEngine, self)._check(res)
-        if (res[:, 7] != 0).any():
-            raise _lib.B2Error("GBOP backup queue overflow: raise queue_factor")
+    def _result(self):
+        res = super(GBOPEngine, self)._result()
+        while (res[:, 7] != 0).any():
+            self.cfg.queue_capacity = grown_queue_capacity(self.queue_capacity, "GBOP")
+            self.workspace = None
+            self._alloc_workspace()
+            self.relaunches += 1
+            self.plan(self._roots)
+            res = super(GBOPEngine, self)._result()
+        return res
 
     def state_values(self, tree=0):
         off = tree * self.ws_per_tree
@@ -55,7 +93,8 @@ class GBOPEngine(HostTieEngine):
 
 
 class GBOPDEngine(TreeEngine):
-    """n_trees independent GBOP-D decisions per launch (GraphBasedPlanner, one warp per decision)."""
+    """n_trees independent GBOP-D decisions per launch (GraphBasedPlanner, one warp per decision).
+    queue_factor: the first backup queue size per tree, in multiples of the state count (grown on overflow)."""
 
     def __init__(self, n_trees, n_actions, budget, gamma, mdp, accuracy=1e-2, sampling_timeout=100, device="cuda",
                  queue_factor=256):
@@ -73,25 +112,40 @@ class GBOPDEngine(TreeEngine):
         self.rev_idx = torch.as_tensor(pairs[:, 1].astype(np.int32), device=self.device)
         self.timeout = int(sampling_timeout)
         gamma = float(gamma)
-        self.queue_capacity = int(queue_factor) * S
         self.cfg = _lib.GBOPDConfig(self.n_trees, self.n_actions, int(budget) // self.n_actions, self.timeout, self.timeout,
-                                    self.queue_capacity, gamma, 1 / (1 - gamma), float(accuracy), self.tables.struct(),
-                                    self.rev_ptr.data_ptr(), self.rev_idx.data_ptr())
+                                    min(int(queue_factor) * S, QUEUE_CAPACITY_MAX), gamma, 1 / (1 - gamma),
+                                    float(accuracy), self.tables.struct(), self.rev_ptr.data_ptr(), self.rev_idx.data_ptr())
         self.lower = torch.empty((self.n_trees, S), dtype=torch.float64, device=self.device)
         self.upper = torch.empty((self.n_trees, S), dtype=torch.float64, device=self.device)
         self.flags = torch.empty((self.n_trees, S), dtype=torch.uint8, device=self.device)
         self.queue = torch.empty((self.n_trees, self.queue_capacity), dtype=torch.int32, device=self.device)
         self.plan_buf = torch.empty((self.n_trees, self.timeout), dtype=torch.int8, device=self.device)
+        self.relaunches = 0          # searches run again after a queue overflow, over the engine's life
+        self._roots = self._rng_words = None
+
+    @property
+    def queue_capacity(self):
+        return int(self.cfg.queue_capacity)
 
     def plan(self, root_states, rng_words):
+        # kept for a relaunch after a queue overflow: the kernel advances the device copy of the words in place
+        self._roots, self._rng_words = root_states, np.array(rng_words, copy=True)
         self._load_rng(rng_words)
         _lib.check(self.lib.b2_gbopd_plan(self.cfg, _lib.ptr(root_states), _lib.ptr(self.lower), _lib.ptr(self.upper),
                                           _lib.ptr(self.flags), _lib.ptr(self.queue), _lib.ptr(self.rng),
                                           _lib.ptr(self.plan_buf), _lib.ptr(self.result), _lib.current_stream()))
 
-    def _check(self, res):
-        if (res[:, 7] != 0).any():
-            raise _lib.B2Error("GBOP-D backup queue overflow: raise queue_factor")
+    def _result(self):
+        res = super(GBOPDEngine, self)._result()
+        while (res[:, 7] != 0).any():
+            self.cfg.queue_capacity = grown_queue_capacity(self.queue_capacity, "GBOP-D")
+            self.queue = None
+            self.queue = self.torch.empty((self.n_trees, self.queue_capacity), dtype=self.torch.int32,
+                                          device=self.device)
+            self.relaunches += 1
+            self.plan(self._roots, self._rng_words)
+            res = super(GBOPDEngine, self)._result()
+        return res
 
     def _plans(self, res):
         """The plan words up to result word 5."""

@@ -45,6 +45,10 @@ class TreeEngine(object):
         """rng_words: uint64 [n_trees, 6] (pcg64_words per tree)."""
         self.rng.copy_(self.torch.from_numpy(np.ascontiguousarray(rng_words).view(np.int64)))
 
+    def _result(self):
+        """Synchronise; -> the result words [n_trees, words] as a numpy array."""
+        return self.result.cpu().numpy()
+
     def _check(self, res):
         """Raise what the reference raises for an error the result words report."""
 
@@ -54,7 +58,7 @@ class TreeEngine(object):
 
     def finish(self):
         """Synchronise; -> (plans, result words [n_trees, words], PCG64 words after the search)."""
-        res = self.result.cpu().numpy()
+        res = self._result()
         self._check(res)
         return self._plans(res), res, self.rng.cpu().numpy().view(np.uint64)
 
@@ -87,7 +91,7 @@ class HostTieEngine(TreeEngine):
     def finish(self, np_randoms=None):
         """Synchronise; -> (plans, result words).  A tie in get_plan is broken on the host with the planner's RNG
         (np_randoms[tree]; default: a fresh generator) exactly as abstract.py:304-311 does."""
-        res = self.result.cpu().numpy()
+        res = self._result()
         self._check(res)
         plans_dev = self.plan_buf.cpu().numpy()
         plans = []
