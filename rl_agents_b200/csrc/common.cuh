@@ -72,4 +72,9 @@ __device__ __forceinline__ double warp_max_f64(double v) {
     return v;
 }
 
+// One step of numpy's max / min reduction (ndarray.max, np.min): a NaN operand wins, so a NaN anywhere in the reduced
+// axis makes the result NaN, whatever its position.  On other operands these are `x > m ? x : m` / `x < m ? x : m`.
+__device__ __forceinline__ double np_max(double m, double x) { return (x > m || isnan(x)) ? x : m; }
+__device__ __forceinline__ double np_min(double m, double x) { return (x < m || isnan(x)) ? x : m; }
+
 }  // namespace b2

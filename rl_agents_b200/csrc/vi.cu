@@ -148,10 +148,7 @@ __global__ void __launch_bounds__(256, 4) vi_sweep_gather_kernel(SweepArgs g) {
         // phase 3: V' = max_a Q'
         for (int s = tid; s < ns; s += 256) {
             double m = qs[s * g.A];
-            for (int a = 1; a < g.A; ++a) {
-                double x = qs[s * g.A + a];
-                m = x > m ? x : m;
-            }
+            for (int a = 1; a < g.A; ++a) m = np_max(m, qs[s * g.A + a]);
             g.v_out[g.row_begin + s0 + s] = m;
         }
         __syncthreads();
@@ -227,10 +224,7 @@ __global__ void __launch_bounds__(256) vi_sweep_row_kernel(SweepArgs g) {
         }
         // V' = max_a Q': the A actions of a state sit in A consecutive lanes
         double m = q;
-        for (int o = 1; o < A; o <<= 1) {
-            const double w = __shfl_xor_sync(0xffffffffu, m, o);
-            m = w > m ? w : m;
-        }
+        for (int o = 1; o < A; o <<= 1) m = np_max(m, __shfl_xor_sync(0xffffffffu, m, o));
         if (live && (qi % A) == 0) g.v_out[g.row_begin + qi / A] = m;
     }
     bad = __reduce_add_sync(0xffffffffu, bad);
@@ -289,7 +283,7 @@ __global__ void vi_rowmax_kernel(SweepArgs g) {
     if (s >= g.rows) return;
     const double* q = g.q_new + s * g.A;
     double m = q[0];
-    for (int a = 1; a < g.A; ++a) m = q[a] > m ? q[a] : m;
+    for (int a = 1; a < g.A; ++a) m = np_max(m, q[a]);
     g.v_out[g.row_begin + s] = m;
 }
 
@@ -321,7 +315,7 @@ __global__ void __launch_bounds__(128) vi_robust_kernel(SweepArgs g, RobustArgs 
                 nv = g.v_in[((const int32_t*)ra.transition)[(int64_t)m * n_rows + row]];
             }
             const double qm = ra.reward[(int64_t)m * n_rows + row] + g.gamma * nv;
-            q = qm < q ? qm : q;                       // np.min over the model axis
+            q = np_min(q, qm);                         // np.min over the model axis
         }
         if (!np_isclose(g.q_old[row], q, g.rtol, g.atol)) bad = 1;
         g.q_new[row] = q;
@@ -388,8 +382,10 @@ extern "C" int b2_vi_sweep(const b2_vi_problem* p, const double* v_in, const dou
     if (tile < 1) tile = 1;
     g.tile_states = tile;
     const size_t smem = ((size_t)tile * E + (size_t)tile * g.A) * sizeof(double);
-    // per device and cheap: set on every call (a process may drive several devices)
-    B2_CUDA_CHECK(cudaFuncSetAttribute(vi_sweep_gather_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+    // at most (8192 + 8192) doubles = 128 KB: tile * E <= max(4096, E) and tile * A <= max(2048, A), E <= 8192
+    // (one state of A = 8192, B = 1).  Per device and cheap: set on every call (a process may drive several devices)
+    B2_CUDA_CHECK(cudaFuncSetAttribute(vi_sweep_gather_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       2 * 8192 * (int)sizeof(double)));
     const int64_t n_tiles = (g.rows + tile - 1) / tile;
     const int64_t max_grid = (int64_t)sm_count() * 8;
     const unsigned grid = (unsigned)(n_tiles < max_grid ? n_tiles : max_grid);

@@ -128,10 +128,7 @@ __global__ void __launch_bounds__(256) vi_sweep_row_p2p_kernel(P2PSweep g) {
                 __stcs(g.q_new + qi, q);
             }
             double m = q;
-            for (int o = 1; o < A; o <<= 1) {
-                const double w = __shfl_xor_sync(0xffffffffu, m, o);
-                m = w > m ? w : m;
-            }
+            for (int o = 1; o < A; o <<= 1) m = np_max(m, __shfl_xor_sync(0xffffffffu, m, o));
             // the exchange step: V'[s] into every rank's copy (own copy first)
             if (live && (qi % A) == 0) {
                 const int64_t s = g.row_begin + qi / A;

@@ -58,6 +58,17 @@ def main():
         q4, sweeps4 = dvi4.solve(60)
         out["vi_p2p_ok_%d" % rep] = bool(np.array_equal(q4.cpu().numpy(), qp_ref[bp:ep])) and sweeps4 == sweeps_p_ref
     dvi4.close()
+    # the same exchange on an MDP with +-inf rewards and zero probabilities: the NaN that numpy's max over actions
+    # keeps crosses the slabs within 3 sweeps (NaN matches any NaN, every other value bit for bit)
+    from tests import vi_cases
+    Pn, Rn, termn, Nn = vi_cases.nonfinite_mdp("sparse", S2, A2, B2, seed=8)
+    with np.errstate(invalid="ignore", over="ignore"):
+        qn_ref, sweeps_n_ref = planners.value_iteration("sparse", Pn, Rn, termn, 0.9, 3, nxt=Nn)
+    dvi5 = DistributedVI("sparse", Pn, Rn, termn, nxt=Nn, gamma=0.9, device=dev, exchange="p2p", max_iterations=8)
+    qn, sweeps_n = dvi5.solve(3)
+    out["vi_p2p_nonfinite_ok"] = bool(np.array_equal(qn.cpu().numpy(), qn_ref[bp:ep], equal_nan=True)) \
+        and sweeps_n == sweeps_n_ref
+    dvi5.close()
     # --- root-parallel MCTS: one all-reduce of root statistics ---
     words = oenvs.make_highway_state(3).pack()
     ss = np.random.SeedSequence(11).spawn(world)[rank]

@@ -27,6 +27,7 @@ def test_two_rank_vi_and_root_parallel_mcts():
     assert all(r["vi_ok"] for r in res)
     assert all(r["vi_local_ok"] for r in res) and all(r["vi_check_every_ok"] for r in res)
     assert all(r["vi_p2p_ok_0"] and r["vi_p2p_ok_1"] for r in res)
+    assert all(r["vi_p2p_nonfinite_ok"] for r in res)
     assert res[0]["vi_sweeps"] == res[1]["vi_sweeps"] < 80          # converged early, same sweep on both ranks
     # every episode of both trees counted once; the episode that expands a root descends into no child
     assert res[0]["mcts_total"] == res[1]["mcts_total"] == 64.0 - 2
