@@ -251,7 +251,8 @@ typedef struct b2_opd_wave_config {
                                robust.py:9-47): root_state / tree.state hold M states per node ([M] ids or
                                [M,136] words), children follow the union of the models' available actions in
                                ascending order, a node's bounds are the minima over the models of the per-model
-                               path bounds (deterministic.py:52-59 with vector rewards)            */
+                               path bounds (deterministic.py:52-59 with vector rewards).  Finite MDPs,
+                               HighwayLite and IntersectionLite; b2_opd_plan_spec takes 0 only     */
     const double* gamma_pow;      /* [n_expansions+2] gamma**d               */
     const double* gamma_pow_div;  /* [n_expansions+2] gamma**d / (1 - gamma) */
     const double* terminal_bonus; /* [n_expansions+2] terminal_reward * gamma**d / (1 - gamma) (:60-63) */

@@ -128,6 +128,8 @@ __device__ __forceinline__ void block_scan2(int a, int b, SelShared& sh, int& ea
 
 // CTA 0: lay out the children of the k chosen leaves (exp_order[n_expanded .. n_expanded + k), id order):
 // child ids by prefix sum of the available-action counts, parent records, work list.
+// JOINT_IL: IntersectionLite with n_models > 0 (see opd_wave_kernel).
+template <bool JOINT_IL>
 __device__ int layout_wave(const Args& a, SelShared& sh, unsigned long long* skeys, bool resident, int n_nodes,
                            int n_expanded, int k, int slot, long long* prof) {
     const int tid = threadIdx.x;
@@ -160,7 +162,7 @@ __device__ int layout_wave(const Args& a, SelShared& sh, unsigned long long* ske
                     if (act_i >= 5) break;
                     const int order[5] = {hw::A_IDLE, hw::A_LEFT, hw::A_RIGHT, hw::A_FASTER, hw::A_SLOWER};
                     act = order[act_i];
-                } else if (a.cfg.env_kind == B2_ENV_INTERSECTION) {
+                } else if (a.cfg.env_kind == B2_ENV_INTERSECTION && !JOINT_IL) {
                     if (act_i >= 3) break;
                     const int order[3] = {il::A_IDLE, il::A_FASTER, il::A_SLOWER};
                     act = order[act_i];
@@ -380,6 +382,7 @@ __device__ int select_dist(const Args& a, SelShared& sh, unsigned long long* ske
 // CTA 0: choose this wave's leaves and lay out their children.  Returns the number of children (0: done).
 // `sel_out` / `do_layout`: the speculative kernel takes the chosen leaves (id order) in its own array and lays the
 // wave out itself; it then returns k.
+template <bool JOINT_IL = false>
 __device__ int select_wave(const Args& a, SelShared& sh, unsigned long long* skeys, int n_nodes, int n_expanded,
                            int staged_nodes, long long* prof, int32_t* sel_out = nullptr, bool do_layout = true) {
     const int tid = threadIdx.x;
@@ -541,7 +544,7 @@ __device__ int select_wave(const Args& a, SelShared& sh, unsigned long long* ske
     __syncthreads();
     if (tid == 0) prof[2] += clock64() - t0;
     if (!do_layout) return k;
-    return layout_wave(a, sh, skeys, resident, n_nodes, n_expanded, k, slot, prof);
+    return layout_wave<JOINT_IL>(a, sh, skeys, resident, n_nodes, n_expanded, k, slot, prof);
 }
 
 // node record of a new child: DeterministicNode.__init__ / update (deterministic.py:10-19, 45-63)
@@ -691,6 +694,9 @@ __device__ void finish_tree(const Args& a, long long tp) {
     }
 }
 
+// JOINT_IL: DROP on IntersectionLite (env_kind INTERSECTION, n_models > 0), an instantiation of its own so that every
+// other configuration, plain IntersectionLite included, runs the same code as without it.
+template <bool JOINT_IL>
 __global__ void __launch_bounds__(THREADS, 1) opd_wave_kernel(Args a) {
     extern __shared__ unsigned long long skeys[];
     __shared__ SelShared sh;
@@ -704,7 +710,11 @@ __global__ void __launch_bounds__(THREADS, 1) opd_wave_kernel(Args a) {
         // root: DeterministicNode.__init__ (:10-19)
         int avail = 0;
         const int Mx = a.cfg.n_models > 0 ? a.cfg.n_models : 1;
-        if (a.cfg.env_kind == B2_ENV_INTERSECTION) {
+        if (JOINT_IL) {
+            for (int i = tid; i < Mx * il::WORDS; i += THREADS) tr.state[i] = a.root_state[i];
+            for (int m = 0; m < Mx; ++m)      // JointEnv.get_available_actions: the union over the models
+                avail |= il::avail_mask(a.root_state[m * il::WORDS + 129]);
+        } else if (a.cfg.env_kind == B2_ENV_INTERSECTION) {
             for (int i = tid; i < il::WORDS; i += THREADS) tr.state[i] = a.root_state[i];
             avail = il::avail_mask(a.root_state[129]);
         } else if (hwy) {
@@ -746,7 +756,7 @@ __global__ void __launch_bounds__(THREADS, 1) opd_wave_kernel(Args a) {
             lap(1);
             if (blockIdx.x == 0) {
                 int children = 0;
-                if (k > 0) children = layout_wave(a, sh, skeys, false, nn, ne, k, 0, ctl->prof);
+                if (k > 0) children = layout_wave<JOINT_IL>(a, sh, skeys, false, nn, ne, k, 0, ctl->prof);
                 if (tid == 0) {
                     if (children == 0) ctl->stop = 1;
                     tp = clock64();
@@ -756,7 +766,7 @@ __global__ void __launch_bounds__(THREADS, 1) opd_wave_kernel(Args a) {
         } else if (blockIdx.x == 0) {
             const int nn = s_nodes, ne = s_expanded, ns = s_staged;
             __syncthreads();
-            const int children = select_wave(a, sh, skeys, nn, ne, ns, ctl->prof);
+            const int children = select_wave<JOINT_IL>(a, sh, skeys, nn, ne, ns, ctl->prof);
             if (tid == 0) {
                 if (children == 0) ctl->stop = 1;
                 else { s_staged = nn; s_nodes = ctl->n_nodes; s_expanded = ctl->n_expanded; }
@@ -797,7 +807,7 @@ __global__ void __launch_bounds__(THREADS, 1) opd_wave_kernel(Args a) {
                     }
                 }
             }
-        } else if (a.cfg.env_kind == B2_ENV_INTERSECTION) {
+        } else if (a.cfg.env_kind == B2_ENV_INTERSECTION && !JOINT_IL) {
             const int warp_global = (tid >> 5) * (int)n_ctas + (int)blockIdx.x;
             const int n_warps = WARPS * (int)n_ctas;
             for (int w0 = 2 * warp_global; w0 < total; w0 += 2 * n_warps) {
@@ -815,6 +825,29 @@ __global__ void __launch_bounds__(THREADS, 1) opd_wave_kernel(Args a) {
                     const int c = base + w;
                     il::store_state(tr.state + (int64_t)c * il::WORDS, li, L, g);
                     if (li == 0) write_child(a, c, leaf, action, (double)r, term, il::avail_mask(g.si));
+                }
+            }
+        } else if (JOINT_IL) {
+            // joint mode: one (child, model) per 16-lane group, the model's scene at (node * M + m) * WORDS
+            const int warp_global = (tid >> 5) * (int)n_ctas + (int)blockIdx.x;
+            const int n_warps = WARPS * (int)n_ctas;
+            const int n_tasks = total * M;
+            for (int w0 = 2 * warp_global; w0 < n_tasks; w0 += 2 * n_warps) {
+                const int task_raw = w0 + ((tid >> 4) & 1);
+                const bool real = task_raw < n_tasks;
+                const int task = real ? task_raw : w0;
+                const int w = task / M, m = task - w * M;
+                const int item = __ldcg(a.work + w);
+                const int leaf = item & 0x0fffffff, action = real ? (item >> 28) & 7 : il::A_IDLE;
+                il::Lane L;
+                il::Globals g;
+                il::load_state<true>(tr.state + ((int64_t)leaf * M + m) * il::WORDS, li, L, g);
+                bool term, trunc;
+                const float r = il::step(L, li, g, action, term, trunc, 0xffffffffu);
+                if (real) {
+                    const int c = base + w;
+                    il::store_state(tr.state + ((int64_t)c * M + m) * il::WORDS, li, L, g);
+                    if (li == 0) write_model_bounds(a, task, c, leaf, m, (double)r, term, il::avail_mask(g.si));
                 }
             }
         } else if (M > 0) {
@@ -1209,7 +1242,7 @@ extern "C" int b2_opd_plan_wave(const b2_opd_wave_config* cfg, const int32_t* ro
     } else if (cfg->env_kind == B2_ENV_HIGHWAY) {
         B2_REQUIRE(cfg->n_actions == B2_HW_ACTIONS, "HighwayLite has 5 actions");
     } else if (cfg->env_kind == B2_ENV_INTERSECTION) {
-        B2_REQUIRE(cfg->n_actions == B2_IL_ACTIONS && cfg->n_models == 0, "IntersectionLite has 3 actions (no joint mode)");
+        B2_REQUIRE(cfg->n_actions == B2_IL_ACTIONS, "IntersectionLite has 3 actions");
     } else {
         set_error("unknown env_kind %d", cfg->env_kind);
         return B2_ERR_INVALID;
@@ -1234,16 +1267,18 @@ extern "C" int b2_opd_plan_wave(const b2_opd_wave_config* cfg, const int32_t* ro
     B2_CUDA_CHECK(cudaMemsetAsync(a.dscr, 0, sizeof(wave::DistScratch), stream));
     const int stage = cfg->node_capacity < wave::STAGE_CAP ? cfg->node_capacity : wave::STAGE_CAP;
     const size_t smem = (size_t)stage * 8;
-    B2_CUDA_CHECK(cudaFuncSetAttribute(wave::opd_wave_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const void* kernel = cfg->env_kind == B2_ENV_INTERSECTION && cfg->n_models > 0 ? (const void*)wave::opd_wave_kernel<true>
+                                                                                    : (const void*)wave::opd_wave_kernel<false>;
+    B2_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int per_sm = 0;
-    B2_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, wave::opd_wave_kernel, wave::THREADS, smem));
+    B2_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, wave::THREADS, smem));
     B2_REQUIRE(per_sm >= 1, "wave kernel does not fit on an SM");
     // one CTA per SM; a wave of w children keeps ceil(w / 16) CTAs busy, the others only pass the barriers
     int grid = sm_count();
     if (cfg->max_ctas > 0 && cfg->max_ctas < grid) grid = cfg->max_ctas;
     if (grid > wave::THREADS) grid = wave::THREADS;      // the distributed selection scans the CTA table with one block
     void* params[] = {&a};
-    B2_CUDA_CHECK(cudaLaunchCooperativeKernel((const void*)wave::opd_wave_kernel, dim3(grid), dim3(wave::THREADS), params,
+    B2_CUDA_CHECK(cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(wave::THREADS), params,
                                               smem, stream));
     return B2_OK;
 }

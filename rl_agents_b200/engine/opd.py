@@ -93,7 +93,8 @@ class OPDWaveEngine(_OPDWholeGPU):
     def __init__(self, env_kind, n_actions, budget, gamma, width, terminal_reward=0.0, mdp=None, device="cuda",
                  max_ctas=0, n_models=0, model_mdps=None):
         """n_models = M >= 1: DROP (DiscreteRobustPlanner, rl_agents/agents/robust/robust.py) -- the joint env of M
-        models; `model_mdps`: the M finite MDPs (env_kind FINITE), root states [M] ids or [M, 136] words."""
+        models; `model_mdps`: the M finite MDPs (env_kind FINITE), root states [M] ids or [M, 136] words (HighwayLite or
+        IntersectionLite scenes, one per model)."""
         first = model_mdps[0] if (model_mdps and env_kind == _lib.ENV_FINITE) else mdp
         super(OPDWaveEngine, self).__init__(env_kind, n_actions, budget, gamma, width, terminal_reward, first, device,
                                             max_ctas, n_models)

@@ -1,6 +1,7 @@
 """IntersectionLite env (docs/INTERSECTION_LITE_SPEC.md): host-side container of one scene (136 32-bit words) with a
 gymnasium-style API -- the repo's model of BASELINE config C5's `intersection-v0`.  `step` runs the CUDA transition
-(b2_intersection_step), the same device code the wavefront OPD kernel expands nodes with."""
+(b2_intersection_step), the same device code the wavefront OPD kernel expands nodes with.  `set_route_at_intersection`
+makes the route-hypothesis copies DROP plans over (spec "Route hypotheses"), in numpy on the host."""
 import copy
 
 import numpy as np
@@ -8,6 +9,8 @@ import numpy as np
 from rl_agents_b200 import _lib
 
 V_SLOTS, N_ACTIONS, N_ROUTES = 16, 3, 12
+N_TURNS = 3
+APPROACH = np.float32(40.0)          # the box edge: vehicles with s < APPROACH are still on their entry's approach
 ACTIONS = {0: "SLOWER", 1: "IDLE", 2: "FASTER"}
 
 
@@ -34,6 +37,30 @@ def make_scene(seed, n_others=8):
         next_s[e] = s0 + f32(12.0)
         f[k], f[16 + k], w[32 + k], w[48 + k] = f32(s0), f32(rng.uniform(6.0, 9.0)), route, 1
     w[128], w[129], w[130], w[131], w[132] = 0, 1, 0, int(rng.integers(0, 1000)), 0
+    return w
+
+
+def route_hypothesis(words, _to):
+    """The scene `words` (left untouched) with every present other vehicle still on its approach (slot >= 1,
+    s < 40) turned towards `_to`: an integer turn (0 left, 1 straight, 2 right, taken mod 3) or "random" (a turn
+    hashed from t, the slot and spawn_seq).  Raises ValueError on any other argument."""
+    if isinstance(_to, str) and _to == "random":
+        turn = None
+    elif isinstance(_to, (int, np.integer)) and not isinstance(_to, (bool, np.bool_)):
+        turn = int(_to) % N_TURNS
+    else:
+        raise ValueError("set_route_at_intersection takes an integer turn or \"random\", got %r" % (_to,))
+    w = np.array(words, dtype=np.int32)
+    s = w[0:V_SLOTS].view(np.float32)
+    t, seq = int(w[128]), int(w[131])
+    for k in range(1, V_SLOTS):
+        if not (w[48 + k] & 1) or not s[k] < APPROACH:
+            continue
+        k_turn = turn
+        if turn is None:
+            h = ((t * 16 + k) * 2654435761 + seq * 40503) & 0xffffffff
+            k_turn = (h >> 16) % N_TURNS
+        w[32 + k] = N_TURNS * (int(w[32 + k]) // N_TURNS) + k_turn
     return w
 
 
@@ -71,6 +98,13 @@ class IntersectionLiteEnv(object):
 
     def get_available_actions(self):
         return available_actions(self.words)
+
+    def set_route_at_intersection(self, _to):
+        """A copy of the env in which the other vehicles still on their approach take the exit `_to` (0 left,
+        1 straight, 2 right, mod 3) or "random"; the env itself is unchanged (route_hypothesis)."""
+        env = copy.deepcopy(self)
+        env.words = route_hypothesis(self.words, _to)
+        return env
 
     def observation(self):
         f = self.words[:32].view(np.float32).reshape(2, V_SLOTS)
