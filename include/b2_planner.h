@@ -496,8 +496,10 @@ int b2_olop_plan(const b2_olop_config* cfg, const int32_t* root_states, const b2
                  uint64_t* rng, int8_t* plan, int32_t* result, void* stream);
 
 /* ------------------------------------------------------------------------
- * MDP-GapE -- rl_agents/agents/tree_search/mdp_gape.py (KL upper bound; deterministic env models, so only
- * one next state per chance node is ever observed)
+ * MDP-GapE -- rl_agents/agents/tree_search/mdp_gape.py (KL upper bound).  b2_mdp_gape_plan runs the deterministic
+ * env models, where a chance node only ever observes one next state; b2_mdp_gape_plan_sampled runs finite MDPs in
+ * every mode, where a chance node observes up to max_next_states distinct next states and its backup solves the
+ * KL-constrained expectation (utils.py:292-342) by Newton's method.
  * ---------------------------------------------------------------------- */
 typedef struct b2_mdp_gape_config {
     int32_t env_kind;
@@ -517,8 +519,9 @@ typedef struct b2_mdp_gape_config {
 } b2_mdp_gape_config;
 
 /* One arena for decision and chance nodes; node id = creation order (placeholders in index order, chance nodes in
- * available-action order).  The children of a chance node are its placeholders fc .. fc+K-1; the observed one is
- * fc, which the reference moves to the end of its child order. */
+ * available-action order).  The children of a chance node are its placeholders fc .. fc+K-1.  The i-th distinct next
+ * state observed takes placeholder fc+i, so a chance node with n observed states orders its children as the reference
+ * does: fc+n .. fc+K-1, then fc .. fc+n-1 (b2_mdp_gape_plan: n = 1). */
 typedef struct b2_mdp_gape_tree {
     int32_t* parent;
     int32_t* first_child;
@@ -534,12 +537,28 @@ typedef struct b2_mdp_gape_tree {
 
 #define B2_MDP_GAPE_RESULT_WORDS 8
 /* per tree int32 result: [0] n_nodes [1] episodes run [2] error (1: reward outside [0,1], olop.py:133-134;
- * 2: a single available action at the root -- max() of an empty list in the reference, :247) [3] recommended
- * action [4] best [5] challenger (root children's node ids, UGapE :238-249) */
+ * 2: a single available action at the root -- max() of an empty list in the reference, :247; sampled only --
+ * 3: a chance node observed more than max_next_states distinct next states, the reference's "No more placeholder
+ * nodes available" ValueError, :283-285; 4: a reached probability row that Generator.choice rejects) [3] recommended
+ * action [4] best [5] challenger (root children's node ids, UGapE :238-249) [6] sampled: the rejected row
+ * s * n_actions + a of error 4, else -1; 0 for b2_mdp_gape_plan.  An error stops its own tree only. */
 
 /* MDPGapE.plan (:94-110); rng as in b2_mcts_plan; plan: int8 [n_trees], the recommended action (-1 on error). */
 int b2_mdp_gape_plan(const b2_mdp_gape_config* cfg, const int32_t* root_states, const b2_mdp_gape_tree* tree,
                      uint64_t* rng, int8_t* plan, int32_t* result, void* stream);
+
+/* MDPGapE.plan on a finite MDP in any mode (b2_finite_mdp_sampled is declared with sparse sampling below).
+ * cfg->env_kind must be B2_ENV_FINITE; cfg->mdp is not read.  Every episode seeds the env copy's generator with
+ * default_rng(np_random.randint(2**30)) (:67); with env_draws = 1 ("stochastic" / "sparse") every step draws once
+ * from it (Generator.choice), with 0 (a "deterministic" table, n_next = 1) none.  terminal: uint8 [n_states]; done =
+ * terminal[state before the step].  keys: int32 [n_trees, node_capacity], written: the state id a decision node was
+ * observed under, -1 on unobserved placeholders, the root and chance nodes.  Floats are fp64 in the reference's order,
+ * its dot products as fma chains; only CUDA's log / exp differ from the host's. */
+struct b2_finite_mdp_sampled;
+int b2_mdp_gape_plan_sampled(const b2_mdp_gape_config* cfg, const struct b2_finite_mdp_sampled* mdp,
+                             const uint8_t* terminal, int32_t env_draws, const int32_t* root_states,
+                             const b2_mdp_gape_tree* tree, int32_t* keys, uint64_t* rng, int8_t* plan, int32_t* result,
+                             void* stream);
 
 /* ------------------------------------------------------------------------
  * BRUE -- rl_agents/agents/tree_search/brue.py (deterministic env models, so every chance node has exactly one

@@ -261,6 +261,8 @@ EXPORTS = {
                              c_void_p, c_void_p]),
     "b2_mdp_gape_plan": (c_int, [ctypes.POINTER(MDPGapEConfig), c_void_p, ctypes.POINTER(MDPGapETree), c_void_p,
                                  c_void_p, c_void_p, c_void_p]),
+    "b2_mdp_gape_plan_sampled": (c_int, [ctypes.POINTER(MDPGapEConfig), ctypes.POINTER(FiniteMDPSampled), c_void_p,
+                                         c_int32, c_void_p, ctypes.POINTER(MDPGapETree)] + [c_void_p] * 5),
     "b2_brue_plan": (c_int, [ctypes.POINTER(BRUEConfig), c_void_p, ctypes.POINTER(BRUETree), c_void_p, c_void_p,
                              c_void_p, c_void_p]),
     "b2_sparse_sampling_workspace_bytes": (c_int64, [ctypes.POINTER(SparseSamplingConfig)]),

@@ -1,5 +1,6 @@
 """MDP-GapE agent on the device engine.  Drop-in for
-rl_agents.agents.tree_search.mdp_gape.MDPGapEAgent (mdp_gape.py:11-344) with step_strategy "reset"."""
+rl_agents.agents.tree_search.mdp_gape.MDPGapEAgent (mdp_gape.py:11-344) with step_strategy "reset", on HighwayLite and
+on finite MDPs in every mode ("stochastic" and "sparse" ones with several observed next states per chance node)."""
 import numpy as np
 
 from rl_agents_b200.agents.common.abstract import register_with_reference

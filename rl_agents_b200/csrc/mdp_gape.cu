@@ -6,16 +6,26 @@
 // in-kernel in fp64.
 //
 // The tree alternates decision nodes (value bounds, KL statistics of the reward received on arrival) and chance
-// nodes (one per available action).  A chance node's children are max_next_states_count placeholders; the env
-// models here are deterministic, so only placeholder 0 is ever observed, and it is moved to the END of the
-// chance node's child order (mdp_gape.py:272-286) -- the order in which the backup sums.  Then
+// nodes (one per available action).  A chance node's children are max_next_states_count placeholders.  On the
+// deterministic env models (FiniteEnv, HighwayEnv) only placeholder 0 is ever observed, and it is moved to the END
+// of the chance node's child order (mdp_gape.py:272-286) -- the order in which the backup sums.  Then
 // max_expectation_under_constraint (utils.py:292-342) sees a distribution with one positive element and needs
 // no Newton solve: it is restated operation by operation in gape_expectation().
+//
+// SampledFiniteEnv steps a finite MDP in any mode with the episode's env generator default_rng(seed), one
+// Generator.choice per step.  A chance node then observes up to max_next_states_count distinct next states, keyed
+// by state id (keys[]): the i-th one takes placeholder i, so the dict order is the placeholders n .. K-1, then the
+// observed 0 .. n-1.  Its backup runs max_expectation_under_constraint in full (gape_expectation_kl(), the Newton
+// solve included).  The reference's 1-D dot products are sequential fused multiply-add chains from 0.0 (numpy's and
+// numba's `@` on the host for lengths up to 15); the library builds with -fmad=false, so they are written with
+// explicit fma() and every other operation stays unfused, in the reference's order.
 //
 // Same lane-group mapping as olop.cu: one tree per 16-lane group (HighwayLite, lane = vehicle slot) or per lane
 // (finite MDP).  Every lane of a group holds a copy of the tree's RNG and takes every selection decision
 // itself from the tree arrays; lane 0 writes the tree.  A tree whose stopping rule fired leaves its episode
 // loop; hw::step only synchronises the 16 lanes of one group, so the other trees of the warp carry on.
+#include <type_traits>
+
 #include "common.cuh"
 #include "kl_bound.cuh"
 #include "lane_env.cuh"
@@ -26,6 +36,7 @@ namespace {
 
 constexpr int KIND_DECISION = 0, KIND_CHANCE = 1;
 constexpr int DONE_BIT = 1 << 16, KIND_SHIFT = 17;
+constexpr int ERR_PLACEHOLDERS = 3, ERR_BAD_ROW = 4;
 
 struct GapeArgs {
     b2_mdp_gape_config cfg;
@@ -34,7 +45,25 @@ struct GapeArgs {
     uint64_t* rng;
     int8_t* plan;
     int32_t* result;
+    // SampledFiniteEnv only
+    b2_finite_mdp_sampled smdp;
+    const uint8_t* terminal;
+    int32_t* keys;
+    int32_t env_draws;
 };
+
+// A finite MDP in any mode, stepped as FiniteMDPEnv.step with the episode's env generator (env_rng)
+struct SampledFiniteEnv {
+    static constexpr int GROUP = 1;
+    int s;
+    Pcg64 env_rng;
+    __device__ __forceinline__ void load_root(const int32_t* root_states, int tree, int li) { s = root_states[tree]; }
+    __device__ __forceinline__ int avail(int n_actions, unsigned gmask) const { return (1 << n_actions) - 1; }
+    __device__ __forceinline__ static int nth(int mask, int n) { return n; }
+};
+
+template <class Env>
+constexpr bool kSampled = std::is_same<Env, SampledFiniteEnv>::value;
 
 // ChanceNode.backup_to_root (mdp_gape.py:288-305) for one side: with f = u_next (upper) or -l_next (lower),
 // p = max_expectation_under_constraint(f, p_hat, c) and the bound is p @ (u_next | l_next).  Children in the
@@ -79,6 +108,103 @@ __device__ double gape_expectation(const b2_mdp_gape_tree& tr, int64_t nb, int f
         s = s + p * v;
     }
     return s + p_obs * value(fc);
+}
+
+// ChanceNode.backup_to_root (mdp_gape.py:288-305) for one side, in full: f = u_next (upper) or -l_next (lower),
+// p = max_expectation_under_constraint(f, p_hat, c) (utils.py:292-342) and the bound is p @ (u_next | l_next).
+// The K children fc .. fc+K-1 hold the observed next states 0 .. n-1 (n >= 1, the positive entries of p_hat in the
+// reference's order) and the unobserved placeholders n .. K-1, which come first in the dict order.
+__device__ double gape_expectation_kl(const b2_mdp_gape_tree& tr, int64_t nb, int fc, int K, int n, bool upper_side,
+                                      double gamma, int cnt, double c) {
+    auto value = [&](int i) {
+        const int64_t id = nb + fc + i;
+        return upper_side ? tr.mu_ucb[id] + gamma * tr.upper[id] : tr.mu_lcb[id] + gamma * tr.lower[id];
+    };
+    auto f = [&](int i) { return upper_side ? value(i) : -value(i); };
+    auto q = [&](int i) { return (double)tr.count[nb + fc + i] / (double)cnt; };
+    // theta_func (:279-282): q_p @ log(l - f_p) + log(q_p @ (1 / (l - f_p))) - c
+    auto theta = [&](double l) {
+        double s1 = 0.0, s2 = 0.0;
+        for (int i = 0; i < n; ++i) {
+            const double d = l - f(i), qi = q(i);
+            s1 = fma(qi, log(d), s1);
+            s2 = fma(qi, 1.0 / d, s2);
+        }
+        return s1 + log(s2) - c;
+    };
+    double fp_max = f(0);
+    for (int i = 1; i < n; ++i) {
+        const double fi = f(i);
+        fp_max = fi > fp_max ? fi : fp_max;
+    }
+    double f_star = fp_max;
+    for (int i = n; i < K; ++i) {
+        const double fi = f(i);
+        f_star = fi > f_star ? fi : f_star;
+    }
+    double lambda = 0.0, z = 0.0, share = 0.0;
+    bool moved = false, solved = false;
+    if (f_star > fp_max) {                                   // :317-323: mass z to the best unobserved entries
+        const double theta_star = theta(f_star);
+        if (theta_star < 0.0) {
+            moved = solved = true;
+            lambda = f_star;
+            z = 1.0 - exp(theta_star);
+            int n_max = 0;
+            for (int i = n; i < K; ++i) n_max += f(i) == f_star;
+            share = z / (double)n_max;
+        }
+    }
+    bool close = false;
+    if (!solved) {
+        // np.isclose(f_p, f_p[0]).all() (atol 1e-8, rtol 1e-5): p = q
+        const double f0 = f(0);
+        close = true;
+        for (int i = 1; i < n; ++i) {
+            const double fi = f(i);
+            close = close && ((fabs(fi - f0) <= 1e-8 + 1e-5 * fabs(f0) && isfinite(f0)) || fi == f0);
+        }
+    }
+    if (!solved && !close) {
+        // newton_iteration(theta, d_theta_dl, 1e-2, x0=f_star + 1, a=f_star) (utils.py:150-203), weight 0.9
+        double x = INFINITY, x_next = f_star + 1.0;
+        for (int it = 0; fabs(x - x_next) > 1e-2 && it < 100; ++it) {
+            x = x_next;
+            const double f_x = theta(x);
+            double s1 = 0.0, s2 = 0.0;                       // d_theta_dl_func (:285-289)
+            for (int i = 0; i < n; ++i) {
+                const double inv = 1.0 / (x - f(i)), qi = q(i);
+                s1 = fma(qi, inv, s1);
+                s2 = fma(qi, inv * inv, s2);
+            }
+            // numba's scalar division by zero raises ZeroDivisionError: the finite difference
+            const double df_x = s1 != 0.0 ? s1 - s2 / s1 : (f_x - theta(x - 1e-2)) / 1e-2;
+            if (df_x != 0.0) x_next = x - f_x / df_x;
+            if (x_next < f_star) x_next = 0.9 * f_star + (1.0 - 0.9) * x;
+        }
+        lambda = x_next < f_star ? f_star : x_next;
+    }
+    double beta = 0.0;
+    int n_uni = 0;
+    if (!close) {                                            // :335: beta = (1 - z) / (q_p @ (1 / (lambda - f_p)))
+        double sb = 0.0;
+        for (int i = 0; i < n; ++i) sb = fma(q(i), 1.0 / (lambda - f(i)), sb);
+        beta = (1.0 - z) / sb;
+        if (beta == 0.0)                                     // :336-339
+            for (int i = 0; i < n; ++i) n_uni += f(i) == f_star;
+    }
+    // p @ next in the dict order: placeholders n .. K-1, then the observed 0 .. n-1
+    double s = 0.0;
+    for (int j = 0; j < K; ++j) {
+        const int i = j < K - n ? n + j : j - (K - n);
+        double p;
+        if (i >= n) p = moved && f(i) == f_star ? share : 0.0;
+        else if (close) p = q(i);
+        else if (beta == 0.0) p = f(i) == f_star ? (1.0 - z) / (double)n_uni : 0.0;
+        else p = (beta * q(i)) / (lambda - f(i));
+        s = fma(p, value(i), s);
+    }
+    return s;
 }
 
 // best_arm_identification_selection (mdp_gape.py:228-249) on the children fc .. fc+n-1 (n >= 2): UGapE's best
@@ -136,8 +262,9 @@ __global__ void __launch_bounds__(128, 8) mdp_gape_kernel(GapeArgs a) {
     Pcg64 rng;
     rng.load(a.rng + (int64_t)tree * B2_PCG64_STATE_WORDS);
     if (writer) new_node(tr, nb, 0, -1, 0xff, KIND_DECISION, a.cfg.init_upper[0]);    // DecisionNode(None)
+    if constexpr (kSampled<Env>) { if (writer) a.keys[nb] = -1; }
     __syncwarp(gmask);
-    int n_nodes = 1, error = 0, episode = 0, best = -1, challenger = -1;
+    int n_nodes = 1, error = 0, episode = 0, best = -1, challenger = -1, bad_row = -1;
     bool done = false;
 
     // expand a decision node (mdp_gape.py:162-170): one chance node per available action, env order
@@ -146,6 +273,7 @@ __global__ void __launch_bounds__(128, 8) mdp_gape_kernel(GapeArgs a) {
         if (writer) {
             for (int i = 0; i < n; ++i) new_node(tr, nb, n_nodes + i, node, Env::nth(amask, i), KIND_CHANCE,
                                                   a.cfg.init_upper[depth]);
+            if constexpr (kSampled<Env>) { for (int i = 0; i < n; ++i) a.keys[nb + n_nodes + i] = -1; }
             tr.first_child[nb + node] = n_nodes;
             tr.meta[nb + node] = (tr.meta[nb + node] & ~0xff00) | (n << 8);
         }
@@ -156,7 +284,8 @@ __global__ void __launch_bounds__(128, 8) mdp_gape_kernel(GapeArgs a) {
     while (!done) {                                  // MDPGapE.plan (:94-110)
         Env env;
         env.load_root(a.root_states, tree, li);      // safe_deepcopy_env(state), :98
-        rng.integers(1u << 30);                      // state.seed(np_random.randint(2**30)), :67
+        const uint32_t seed = rng.integers(1u << 30);    // state.seed(np_random.randint(2**30)), :67
+        if constexpr (kSampled<Env>) { if (a.env_draws) env.env_rng.seed_from(seed); }
         if (tr.first_child[nb] < 0) expand_decision(0, env.avail(a.cfg.n_actions, gmask), 0);
         int node = 0;
         for (int h = 0; h < H; ++h) {
@@ -197,18 +326,40 @@ __global__ void __launch_bounds__(128, 8) mdp_gape_kernel(GapeArgs a) {
                 if ((tr.meta[nb + fc + i] & 0xff) == action) { chance = fc + i; break; }
             action = tr.meta[nb + chance] & 0xff;
             bool term, trunc;
-            const double r = env.step(a.cfg.mdp, action, li, gmask, term, trunc);          // :82
-            // ChanceNode.get_child (:272-286): placeholders on the first visit, the observation takes placeholder 0
+            double r;                                                                        // :82
+            if constexpr (kSampled<Env>) {
+                // FiniteMDPEnv.step: Generator.choice rejects the row (a ValueError), or done = terminal[state
+                // BEFORE the transition] and one draw of the env generator picks the next state
+                const b2_finite_mdp_sampled& m = a.smdp;
+                const int64_t row = (int64_t)env.s * m.n_actions + action;
+                if (a.env_draws && !m.row_ok[row]) { error = ERR_BAD_ROW; bad_row = (int)row; break; }
+                term = a.terminal[env.s] != 0;
+                r = m.reward[row];
+                env.s = sampled_next(m, row, a.env_draws != 0, env.env_rng);
+            } else {
+                r = env.step(a.cfg.mdp, action, li, gmask, term, trunc);
+            }
+            // ChanceNode.get_child (:272-286): placeholders on the first visit; a deterministic env observes placeholder 0
             int child = tr.first_child[nb + chance];
             if (child < 0) {
                 child = n_nodes;
                 if (writer) {
                     for (int i = 0; i < K; ++i) new_node(tr, nb, n_nodes + i, chance, i, KIND_DECISION,
                                                           a.cfg.init_upper[h + 1]);
+                    if constexpr (kSampled<Env>) { for (int i = 0; i < K; ++i) a.keys[nb + n_nodes + i] = -1; }
                     tr.first_child[nb + chance] = n_nodes;
                     tr.meta[nb + chance] = (tr.meta[nb + chance] & ~0xff00) | (K << 8);
                 }
                 n_nodes += K;
+            }
+            if constexpr (kSampled<Env>) {
+                // the i-th distinct next state takes placeholder i: the observation's key, else the first free one;
+                // none left is the reference's ValueError
+                int i = 0;
+                while (i < K && a.keys[nb + child + i] >= 0 && a.keys[nb + child + i] != env.s) ++i;
+                if (i == K) { error = ERR_PLACEHOLDERS; break; }
+                child += i;
+                if (writer) a.keys[nb + child] = env.s;
             }
             if (!(r >= 0.0 && r <= 1.0)) { error = 1; break; }                 // olop.py:133-134
             if (writer) {
@@ -248,7 +399,14 @@ __global__ void __launch_bounds__(128, 8) mdp_gape_kernel(GapeArgs a) {
                     }
                     tr.upper[nb + n] = up;
                     tr.lower[nb + n] = lo;
-                } else {                                                         // :288-305
+                } else if constexpr (kSampled<Env>) {                            // :288-305
+                    const int cnt = tr.count[nb + n];
+                    const double c = a.cfg.transition_thresholds[cnt] / (double)cnt;
+                    int obs = 1;
+                    while (obs < k && a.keys[nb + fc + obs] >= 0) ++obs;
+                    tr.upper[nb + n] = gape_expectation_kl(tr, nb, fc, k, obs, true, gamma, cnt, c);
+                    tr.lower[nb + n] = gape_expectation_kl(tr, nb, fc, k, obs, false, gamma, cnt, c);
+                } else {
                     const int cnt = tr.count[nb + n];
                     const double qp = (double)tr.count[nb + fc] / (double)cnt;
                     const double c = a.cfg.transition_thresholds[cnt] / (double)cnt;
@@ -278,7 +436,7 @@ __global__ void __launch_bounds__(128, 8) mdp_gape_kernel(GapeArgs a) {
         res[3] = action;
         res[4] = error ? -1 : best;
         res[5] = error ? -1 : challenger;
-        res[6] = 0;
+        res[6] = kSampled<Env> ? bad_row : 0;
         res[7] = 0;
     }
 }
@@ -308,6 +466,32 @@ extern "C" int b2_mdp_gape_plan(const b2_mdp_gape_config* cfg, const int32_t* ro
         mdp_gape_kernel<FiniteEnv><<<lane_grid(cfg->n_trees, FiniteEnv::GROUP), 128, 0, stream>>>(a);
     else
         mdp_gape_kernel<HighwayEnv><<<lane_grid(cfg->n_trees, HighwayEnv::GROUP), 128, 0, stream>>>(a);
+    B2_CUDA_CHECK(cudaGetLastError());
+    return B2_OK;
+}
+
+extern "C" int b2_mdp_gape_plan_sampled(const b2_mdp_gape_config* cfg, const b2_finite_mdp_sampled* mdp,
+                                        const uint8_t* terminal, int32_t env_draws, const int32_t* root_states,
+                                        const b2_mdp_gape_tree* tree, int32_t* keys, uint64_t* rng, int8_t* plan,
+                                        int32_t* result, void* stream_) {
+    B2_REQUIRE(cfg && mdp && terminal && root_states && tree && keys && rng && plan && result, "null pointer");
+    B2_REQUIRE(cfg->env_kind == B2_ENV_FINITE, "env_kind must be B2_ENV_FINITE");
+    B2_REQUIRE(cfg->n_trees > 0 && cfg->episodes >= 0 && cfg->horizon >= 1, "bad batch / budget");
+    B2_REQUIRE(cfg->n_actions > 0 && cfg->n_actions <= 8, "n_actions must be in 1..8");
+    B2_REQUIRE(mdp->n_actions == cfg->n_actions && mdp->n_states > 0 && mdp->n_next > 0, "finite MDP shape");
+    B2_REQUIRE(mdp->cdf && mdp->next && mdp->reward && mdp->row_ok, "finite MDP tables missing");
+    B2_REQUIRE(env_draws == 0 || env_draws == 1, "env_draws must be 0 or 1");
+    B2_REQUIRE(cfg->max_next_states >= 1 && cfg->max_next_states <= 255, "max_next_states must be in 1..255");
+    B2_REQUIRE((int64_t)cfg->node_capacity >= 1 + ((int64_t)cfg->episodes + 2) * cfg->horizon *
+                                                      (cfg->n_actions + cfg->max_next_states),
+               "node_capacity too small");
+    B2_REQUIRE(cfg->thresholds && cfg->transition_thresholds && cfg->init_upper,
+               "threshold / initial bound tables missing");
+    cudaStream_t stream = (cudaStream_t)stream_;
+    GapeArgs a;
+    a.cfg = *cfg; a.tree = *tree; a.root_states = root_states; a.rng = rng; a.plan = plan; a.result = result;
+    a.smdp = *mdp; a.terminal = terminal; a.keys = keys; a.env_draws = env_draws;
+    mdp_gape_kernel<SampledFiniteEnv><<<lane_grid(cfg->n_trees, 1), 128, 0, stream>>>(a);
     B2_CUDA_CHECK(cudaGetLastError());
     return B2_OK;
 }

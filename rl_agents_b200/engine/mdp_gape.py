@@ -1,8 +1,11 @@
-"""Batched MDP-GapE engine (device side of MDPGapEAgent)."""
+"""Batched MDP-GapE engine (device side of MDPGapEAgent).
+
+A finite MDP in mode "deterministic" runs b2_mdp_gape_plan on FiniteTables; in mode "stochastic" or "sparse" it runs
+b2_mdp_gape_plan_sampled on SampledFiniteTables, where chance nodes observe several next states."""
 import numpy as np
 
 from rl_agents_b200 import _lib
-from rl_agents_b200.engine.tables import FiniteTables
+from rl_agents_b200.engine.tables import FiniteTables, SampledFiniteTables
 from rl_agents_b200.engine.tree_engine import TreeEngine, decode_action
 
 
@@ -15,6 +18,10 @@ def count_table(expression, episodes, horizon, n_actions, confidence):
     for count in range(1, episodes + 3):
         out[count] = eval(expression, dict(scope, count=count))
     return out
+
+
+PLACEHOLDERS_MESSAGE = ("No more placeholder nodes available, we observed more next states than the "
+                        "'max_next_states_count' config")
 
 
 class MDPGapEEngine(TreeEngine):
@@ -40,22 +47,42 @@ class MDPGapEEngine(TreeEngine):
         self.thresholds = table(upper_bound["threshold"])
         self.transition_thresholds = table(upper_bound["transition_threshold"])
         self.init_upper = torch.as_tensor(init_upper, device=self.device)
-        self.tables = FiniteTables(mdp, self.device) if env_kind == _lib.ENV_FINITE else None
+        self.sampled = env_kind == _lib.ENV_FINITE and mdp.mode != "deterministic"
+        self.tables, self.keys = None, None
+        if self.sampled:
+            self.tables = SampledFiniteTables(mdp, self.device)
+            self.terminal = torch.as_tensor(np.ascontiguousarray(mdp.terminal, dtype=np.uint8), device=self.device)
+            self.keys = torch.empty((self.n_trees, self.capacity), dtype=torch.int32, device=self.device)
+        elif env_kind == _lib.ENV_FINITE:
+            self.tables = FiniteTables(mdp, self.device)
         self.tree = _lib.MDPGapETree(*self._alloc_tree(_lib.MDP_GAPE_TREE_FIELDS, self.capacity))
         self.cfg = _lib.MDPGapEConfig(env_kind, self.n_trees, self.n_actions, self.episodes, self.horizon,
                                       self.capacity, self.n_next, 1 if continuation_type == "uniform" else 0, gamma,
                                       float(accuracy), self.thresholds.data_ptr(),
                                       self.transition_thresholds.data_ptr(), self.init_upper.data_ptr(),
-                                      self.tables.struct() if self.tables else _lib.FiniteMDP())
+                                      self.tables.struct() if self.tables and not self.sampled else _lib.FiniteMDP())
         self.plan_buf = torch.empty(self.n_trees, dtype=torch.int8, device=self.device)
 
     def plan(self, root_states, rng_words):
         """root_states: [n_trees] state ids (finite) or [n_trees, 136] words (HighwayLite), on the device."""
         self._load_rng(rng_words)
+        if self.sampled:
+            _lib.check(self.lib.b2_mdp_gape_plan_sampled(
+                self.cfg, self.tables.struct(), _lib.ptr(self.terminal), 1, _lib.ptr(root_states), self.tree,
+                _lib.ptr(self.keys), _lib.ptr(self.rng), _lib.ptr(self.plan_buf), _lib.ptr(self.result),
+                _lib.current_stream()))
+            return
         _lib.check(self.lib.b2_mdp_gape_plan(self.cfg, _lib.ptr(root_states), self.tree, _lib.ptr(self.rng),
                                              _lib.ptr(self.plan_buf), _lib.ptr(self.result), _lib.current_stream()))
 
     def _check(self, res):
+        bad = np.nonzero(res[:, 2] == 4)[0]
+        if bad.size:                                  # a sampled row Generator.choice rejects: numpy's own message
+            p = self.tables.row(int(res[bad[0], 6]))
+            np.random.default_rng(0).choice(p.size, p=p)
+            raise AssertionError("row %d was flagged but Generator.choice accepts it" % int(res[bad[0], 6]))
+        if (res[:, 2] == 3).any():
+            raise ValueError(PLACEHOLDERS_MESSAGE)                                   # mdp_gape.py:283-285
         if (res[:, 2] == 1).any():
             raise ValueError("This planner assumes that all rewards are normalized in [0, 1]")   # olop.py:133-134
         if (res[:, 2] == 2).any():
@@ -63,10 +90,20 @@ class MDPGapEEngine(TreeEngine):
 
     def tree_dict(self, tree=0):
         """Every node array of one tree, in creation order; `action` is the env action of a chance node, the
-        placeholder index of a decision node below one, -1 at the root."""
+        placeholder index of a decision node below one, -1 at the root.  `order` maps each expanded chance node to
+        its children in the reference's dict order (the unobserved placeholders, then the observed ones in the
+        order they were observed); on a sampled MDP `key` is the state id a decision node was observed under, -1
+        elsewhere."""
         n = int(self.result[tree, 0].item())
         out = {k: getattr(self, k)[tree, :n].cpu().numpy() for k in _lib.MDP_GAPE_TREE_FIELDS}
         meta = out["meta"]
         out.update(action=decode_action(meta), n_children=(meta >> 8) & 0xff, done=((meta >> 16) & 1).astype(bool),
                    kind=(meta >> 17) & 1, cumulative_reward=out["cumulative"])
+        if self.sampled:
+            out["key"] = self.keys[tree, :n].cpu().numpy()
+        out["order"] = {}
+        for c in np.nonzero((out["kind"] == 1) & (out["first_child"] >= 0))[0]:
+            fc, k = int(out["first_child"][c]), int(out["n_children"][c])
+            n_obs = int((out["key"][fc:fc + k] >= 0).sum()) if self.sampled else 1
+            out["order"][int(c)] = list(range(fc + n_obs, fc + k)) + list(range(fc, fc + n_obs))
         return out
