@@ -489,11 +489,25 @@ typedef struct b2_olop_tree {
 #define B2_OLOP_RESULT_WORDS 8
 /* per tree int32 result: [0] n_nodes [1] plan_len
  * [2] error (1: reward outside [0,1], olop.py:133-134; 2: "zeros" continuation
- *     with action 0 unavailable -- a KeyError in the reference, :82,:88) */
+ *     with action 0 unavailable -- a KeyError in the reference, :82,:88; sampled
+ *     only -- 3: a reached probability row that Generator.choice rejects)
+ * [3] b2_olop_plan_sampled: the rejected row s * n_actions + a of error 3, else -1;
+ *     not written by b2_olop_plan.  An error stops its own tree only. */
 
 /* OLOP.plan (:94-100); rng and env_kind as in b2_mcts_plan; plan: int8 [n_trees, horizon]. */
 int b2_olop_plan(const b2_olop_config* cfg, const int32_t* root_states, const b2_olop_tree* tree,
                  uint64_t* rng, int8_t* plan, int32_t* result, void* stream);
+
+/* OLOP.plan on a finite MDP in any mode (b2_finite_mdp_sampled is declared with sparse sampling below).
+ * cfg->env_kind must be B2_ENV_FINITE; cfg->mdp is not read.  Every episode seeds the env copy's generator with
+ * default_rng(np_random.randint(2**30)) (:73); with env_draws = 1 ("stochastic" / "sparse") each of the horizon
+ * steps draws once from it (Generator.choice), after a terminal state too; with 0 (a "deterministic" table,
+ * n_next = 1) none.  terminal: uint8 [n_states]; done = terminal[state before the step].  The tree is the same
+ * open-loop tree as b2_olop_plan's; mu_ucb and upper differ from the host's only through CUDA's log. */
+struct b2_finite_mdp_sampled;
+int b2_olop_plan_sampled(const b2_olop_config* cfg, const struct b2_finite_mdp_sampled* mdp, const uint8_t* terminal,
+                         int32_t env_draws, const int32_t* root_states, const b2_olop_tree* tree, uint64_t* rng,
+                         int8_t* plan, int32_t* result, void* stream);
 
 /* ------------------------------------------------------------------------
  * MDP-GapE -- rl_agents/agents/tree_search/mdp_gape.py (KL upper bound).  b2_mdp_gape_plan runs the deterministic

@@ -259,6 +259,8 @@ EXPORTS = {
                                   c_void_p, c_void_p, c_void_p]),
     "b2_olop_plan": (c_int, [ctypes.POINTER(OLOPConfig), c_void_p, ctypes.POINTER(OLOPTree), c_void_p, c_void_p,
                              c_void_p, c_void_p]),
+    "b2_olop_plan_sampled": (c_int, [ctypes.POINTER(OLOPConfig), ctypes.POINTER(FiniteMDPSampled), c_void_p, c_int32,
+                                     c_void_p, ctypes.POINTER(OLOPTree)] + [c_void_p] * 4),
     "b2_mdp_gape_plan": (c_int, [ctypes.POINTER(MDPGapEConfig), c_void_p, ctypes.POINTER(MDPGapETree), c_void_p,
                                  c_void_p, c_void_p, c_void_p]),
     "b2_mdp_gape_plan_sampled": (c_int, [ctypes.POINTER(MDPGapEConfig), ctypes.POINTER(FiniteMDPSampled), c_void_p,

@@ -1,5 +1,6 @@
 """OLOP / KL-OLOP agent on the device engine.  Drop-in for
-rl_agents.agents.tree_search.olop.OLOPAgent (olop.py:11-200)."""
+rl_agents.agents.tree_search.olop.OLOPAgent (olop.py:11-200), on HighwayLite, IntersectionLite and finite MDPs in every
+mode ("stochastic" and "sparse" ones draw a next state at every step of an episode)."""
 from rl_agents_b200.agents.common.abstract import register_with_reference
 from rl_agents_b200.agents.tree_search.abstract import AbstractPlanner, AbstractTreeSearchAgent
 from rl_agents_b200.agents.tree_search.mcts import allocation
@@ -22,6 +23,9 @@ class OLOP(AbstractPlanner):
         if "horizon" not in self.config:                     # olop.py:36-48
             budget = max(self.env.action_space.n, self.config["budget"])
             self.config["episodes"], self.config["horizon"] = allocation(budget, self.config["gamma"])
+        # the reference builds its root OLOPNode here, which reads upper_bound["type"] (olop.py:115): a config whose
+        # "upper_bound" is a bare string, as the shipped FiniteMDPEnv/agents/olop.json has, raises that TypeError
+        self.config["upper_bound"]["type"]
         super(OLOP, self).reset()
 
     def plan(self, state, observation):

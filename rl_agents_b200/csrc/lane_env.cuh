@@ -7,8 +7,11 @@
 // drops truncation).
 //
 // The planners that sample stochastic finite MDPs draw from a b2_finite_mdp_sampled row with searchsorted_right()
-// (sparse_sampling.cu, which seeds a fresh env generator per sample) or step it with sampled_next() (mcts_dpw.cu).
+// (sparse_sampling.cu, which seeds a fresh env generator per sample) or step it with sampled_next() (mcts_dpw.cu,
+// and SampledFiniteEnv in olop.cu and mdp_gape.cu).
 #pragma once
+#include <type_traits>
+
 #include "common.cuh"
 #include "highway_lite.cuh"
 #include "intersection_lite.cuh"
@@ -34,6 +37,20 @@ __device__ __forceinline__ int sampled_next(const b2_finite_mdp_sampled& m, int6
     const int k = draw ? searchsorted_right(m.cdf + row * B, B, env_rng.random()) : 0;
     return m.next[row * B + k];
 }
+
+// A finite MDP in any mode, stepped as FiniteMDPEnv.step with the episode's env generator (env_rng).  It has no
+// step(): the planners step it in place with sampled_next(), after checking row_ok (kSampled<Env> selects that code).
+struct SampledFiniteEnv {
+    static constexpr int GROUP = 1;
+    int s;
+    Pcg64 env_rng;
+    __device__ __forceinline__ void load_root(const int32_t* root_states, int tree, int li) { s = root_states[tree]; }
+    __device__ __forceinline__ int avail(int n_actions, unsigned gmask) const { return (1 << n_actions) - 1; }
+    __device__ __forceinline__ static int nth(int mask, int n) { return n; }
+};
+
+template <class Env>
+constexpr bool kSampled = std::is_same<Env, SampledFiniteEnv>::value;
 
 struct FiniteEnv {
     static constexpr int GROUP = 1;

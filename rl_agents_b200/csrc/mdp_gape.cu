@@ -24,8 +24,6 @@
 // (finite MDP).  Every lane of a group holds a copy of the tree's RNG and takes every selection decision
 // itself from the tree arrays; lane 0 writes the tree.  A tree whose stopping rule fired leaves its episode
 // loop; hw::step only synchronises the 16 lanes of one group, so the other trees of the warp carry on.
-#include <type_traits>
-
 #include "common.cuh"
 #include "kl_bound.cuh"
 #include "lane_env.cuh"
@@ -51,19 +49,6 @@ struct GapeArgs {
     int32_t* keys;
     int32_t env_draws;
 };
-
-// A finite MDP in any mode, stepped as FiniteMDPEnv.step with the episode's env generator (env_rng)
-struct SampledFiniteEnv {
-    static constexpr int GROUP = 1;
-    int s;
-    Pcg64 env_rng;
-    __device__ __forceinline__ void load_root(const int32_t* root_states, int tree, int li) { s = root_states[tree]; }
-    __device__ __forceinline__ int avail(int n_actions, unsigned gmask) const { return (1 << n_actions) - 1; }
-    __device__ __forceinline__ static int nth(int mask, int n) { return n; }
-};
-
-template <class Env>
-constexpr bool kSampled = std::is_same<Env, SampledFiniteEnv>::value;
 
 // ChanceNode.backup_to_root (mdp_gape.py:288-305) for one side: with f = u_next (upper) or -l_next (lower),
 // p = max_expectation_under_constraint(f, p_hat, c) and the bound is p @ (u_next | l_next).  Children in the

@@ -8,12 +8,21 @@
 //
 // Same lane-group mapping as mcts.cu: one tree per 16-lane group (HighwayLite and
 // IntersectionLite, lane = vehicle slot) or per lane (finite MDP).
+//
+// SampledFiniteEnv (b2_olop_plan_sampled) steps a finite MDP in any mode as
+// FiniteMDPEnv.step does: each episode seeds the env copy's generator with the
+// default_rng(seed) of its randint(2**30) draw, and every one of the `horizon`
+// steps draws once with Generator.choice, also after a terminal state.  The
+// tree stays open-loop (keyed on action sequences), so only its statistics and
+// the plan depend on the draws.
 #include "common.cuh"
 #include "kl_bound.cuh"
 #include "lane_env.cuh"
 #include "pcg64.cuh"
 
 namespace b2 {
+
+constexpr int ERR_BAD_ROW = 3;
 
 struct OlopArgs {
     b2_olop_config cfg;
@@ -22,6 +31,10 @@ struct OlopArgs {
     uint64_t* rng;
     int8_t* plan;
     int32_t* result;
+    // SampledFiniteEnv only
+    b2_finite_mdp_sampled smdp;
+    const uint8_t* terminal;
+    int32_t env_draws;
 };
 
 template <class Env>
@@ -46,12 +59,15 @@ __global__ void __launch_bounds__(128, 8) olop_kernel(OlopArgs a) {
         tr.cumulative[nb] = 0.0; tr.mu_ucb[nb] = a.cfg.kl ? 1.0 : INFINITY; tr.upper[nb] = a.cfg.init_upper[0];
     }
     __syncwarp(gmask);
-    int n_nodes = 1, error = 0;
+    int n_nodes = 1, error = 0, bad_row = -1;
 
     for (int ep = 0; ep < a.cfg.episodes; ++ep) {
         Env env;
         env.load_root(a.root_states, tree, li);     // safe_deepcopy_env(state), olop.py:98
-        if (live) rng.integers(1u << 30);            // state.seed(np_random.randint(2**30)), :73
+        if (live) {
+            const uint32_t seed = rng.integers(1u << 30);    // state.seed(np_random.randint(2**30)), :73
+            if constexpr (kSampled<Env>) { if (a.env_draws) env.env_rng.seed_from(seed); }
+        }
         int node = 0;
         const double threshold = a.cfg.thresholds[ep];
         for (int h = 0; h < L; ++h) {
@@ -97,7 +113,27 @@ __global__ void __launch_bounds__(128, 8) olop_kernel(OlopArgs a) {
                 action = tr.meta[nb + child] & 0xff;
             }
             bool term, trunc;
-            const double r = env.step(a.cfg.mdp, action, li, gmask, term, trunc);     // olop.py:87
+            double r;                                                                   // olop.py:87
+            if constexpr (kSampled<Env>) {
+                // FiniteMDPEnv.step: Generator.choice rejects the row (a ValueError), or done = terminal[state
+                // BEFORE the transition] and one draw of the env generator picks the next state
+                r = 0.0;
+                term = false;
+                if (live && !error) {
+                    const b2_finite_mdp_sampled& m = a.smdp;
+                    const int64_t row = (int64_t)env.s * m.n_actions + action;
+                    if (a.env_draws && !m.row_ok[row]) {
+                        error = ERR_BAD_ROW;
+                        bad_row = (int)row;
+                    } else {
+                        term = a.terminal[env.s] != 0;
+                        r = m.reward[row];
+                        env.s = sampled_next(m, row, a.env_draws != 0, env.env_rng);
+                    }
+                }
+            } else {
+                r = env.step(a.cfg.mdp, action, li, gmask, term, trunc);
+            }
             if (live && !error) {
                 node = child;
                 // update (olop.py:132-142)
@@ -159,6 +195,7 @@ __global__ void __launch_bounds__(128, 8) olop_kernel(OlopArgs a) {
         res[0] = n_nodes;
         res[1] = len;
         res[2] = error;
+        if constexpr (kSampled<Env>) res[3] = bad_row;
     }
 }
 
@@ -185,6 +222,29 @@ extern "C" int b2_olop_plan(const b2_olop_config* cfg, const int32_t* root_state
         olop_kernel<HighwayEnv><<<lane_grid(cfg->n_trees, HighwayEnv::GROUP), 128, 0, stream>>>(a);
     else
         olop_kernel<IntersectionEnv><<<lane_grid(cfg->n_trees, IntersectionEnv::GROUP), 128, 0, stream>>>(a);
+    B2_CUDA_CHECK(cudaGetLastError());
+    return B2_OK;
+}
+
+extern "C" int b2_olop_plan_sampled(const b2_olop_config* cfg, const b2_finite_mdp_sampled* mdp,
+                                    const uint8_t* terminal, int32_t env_draws, const int32_t* root_states,
+                                    const b2_olop_tree* tree, uint64_t* rng, int8_t* plan, int32_t* result,
+                                    void* stream_) {
+    B2_REQUIRE(cfg && mdp && terminal && root_states && tree && rng && plan && result, "null pointer");
+    B2_REQUIRE(cfg->env_kind == B2_ENV_FINITE, "env_kind must be B2_ENV_FINITE");
+    B2_REQUIRE(cfg->n_trees > 0 && cfg->episodes >= 0 && cfg->horizon >= 1, "bad batch / budget");
+    B2_REQUIRE(cfg->n_actions > 0 && cfg->n_actions <= 8, "n_actions must be in 1..8");
+    B2_REQUIRE(mdp->n_actions == cfg->n_actions && mdp->n_states > 0 && mdp->n_next > 0, "finite MDP shape");
+    B2_REQUIRE(mdp->cdf && mdp->next && mdp->reward && mdp->row_ok, "finite MDP tables missing");
+    B2_REQUIRE(env_draws == 0 || env_draws == 1, "env_draws must be 0 or 1");
+    B2_REQUIRE((int64_t)cfg->node_capacity >= 1 + (int64_t)cfg->episodes * cfg->horizon * cfg->n_actions,
+               "node_capacity too small");
+    B2_REQUIRE(cfg->thresholds && cfg->init_upper, "threshold / initial bound tables missing");
+    cudaStream_t stream = (cudaStream_t)stream_;
+    OlopArgs a;
+    a.cfg = *cfg; a.tree = *tree; a.root_states = root_states; a.rng = rng; a.plan = plan; a.result = result;
+    a.smdp = *mdp; a.terminal = terminal; a.env_draws = env_draws;
+    olop_kernel<SampledFiniteEnv><<<lane_grid(cfg->n_trees, SampledFiniteEnv::GROUP), 128, 0, stream>>>(a);
     B2_CUDA_CHECK(cudaGetLastError());
     return B2_OK;
 }

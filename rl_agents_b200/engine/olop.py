@@ -1,10 +1,14 @@
-"""Batched OLOP / KL-OLOP engine (device side of OLOPAgent)."""
+"""Batched OLOP / KL-OLOP engine (device side of OLOPAgent).
+
+A finite MDP in mode "deterministic" runs b2_olop_plan on FiniteTables; in mode "stochastic" or "sparse" it runs
+b2_olop_plan_sampled on SampledFiniteTables, where every step of an episode draws its next state from the episode's
+env generator."""
 import logging
 
 import numpy as np
 
 from rl_agents_b200 import _lib
-from rl_agents_b200.engine.tables import FiniteTables
+from rl_agents_b200.engine.tables import FiniteTables, SampledFiniteTables
 from rl_agents_b200.engine.tree_engine import TreeEngine, decode_action
 
 logger = logging.getLogger(__name__)
@@ -42,20 +46,36 @@ class OLOPEngine(TreeEngine):
         self.init_upper = torch.as_tensor(init_upper, device=self.device)
         self.thresholds = torch.as_tensor(thresholds_for(upper_bound, self.episodes) if self.kl
                                           else np.zeros(max(self.episodes, 1)), device=self.device)
-        self.tables = FiniteTables(mdp, self.device) if env_kind == _lib.ENV_FINITE else None
+        self.sampled = env_kind == _lib.ENV_FINITE and mdp.mode != "deterministic"
+        self.tables = None
+        if self.sampled:
+            self.tables = SampledFiniteTables(mdp, self.device)
+            self.terminal = torch.as_tensor(np.ascontiguousarray(mdp.terminal, dtype=np.uint8), device=self.device)
+        elif env_kind == _lib.ENV_FINITE:
+            self.tables = FiniteTables(mdp, self.device)
         self.tree = _lib.OLOPTree(*self._alloc_tree(_lib.OLOP_TREE_FIELDS, self.capacity))
         self.cfg = _lib.OLOPConfig(env_kind, self.n_trees, self.n_actions, self.episodes, self.horizon, self.capacity,
                                    1 if self.kl else 0, 1 if continuation_type == "uniform" else 0, gamma,
                                    self.thresholds.data_ptr(), self.init_upper.data_ptr(),
-                                   self.tables.struct() if self.tables else _lib.FiniteMDP())
+                                   self.tables.struct() if self.tables and not self.sampled else _lib.FiniteMDP())
         self.plan_buf = torch.empty((self.n_trees, max(self.horizon, 1)), dtype=torch.int8, device=self.device)
 
     def plan(self, root_states, rng_words):
         self._load_rng(rng_words)
+        if self.sampled:
+            _lib.check(self.lib.b2_olop_plan_sampled(
+                self.cfg, self.tables.struct(), _lib.ptr(self.terminal), 1, _lib.ptr(root_states), self.tree,
+                _lib.ptr(self.rng), _lib.ptr(self.plan_buf), _lib.ptr(self.result), _lib.current_stream()))
+            return
         _lib.check(self.lib.b2_olop_plan(self.cfg, _lib.ptr(root_states), self.tree, _lib.ptr(self.rng),
                                          _lib.ptr(self.plan_buf), _lib.ptr(self.result), _lib.current_stream()))
 
     def _check(self, res):
+        bad = np.nonzero(res[:, 2] == 3)[0]
+        if bad.size:                                  # a sampled row Generator.choice rejects: numpy's own message
+            p = self.tables.row(int(res[bad[0], 3]))
+            np.random.default_rng(0).choice(p.size, p=p)
+            raise AssertionError("row %d was flagged but Generator.choice accepts it" % int(res[bad[0], 3]))
         if (res[:, 2] == 1).any():
             raise ValueError("This planner assumes that all rewards are normalized in [0, 1]")   # olop.py:133-134
         if (res[:, 2] == 2).any():
