@@ -52,6 +52,20 @@ typedef struct b2_finite_mdp {
     const uint8_t* terminal;   /* [S]                                        */
 } b2_finite_mdp;
 
+/* A finite MDP as the sampled env steps it (FiniteMDPEnv.step): r = reward[s, a]; k = searchsorted(cdf[s, a], u,
+ * "right") for u = default_rng(seed).random(); s' = next[s, a, k]. */
+typedef struct b2_finite_mdp_sampled {
+    int32_t n_states;
+    int32_t n_actions;
+    int32_t n_next;          /* B: 1 "deterministic", S "stochastic" (next[s, a, k] = k), next's width "sparse" */
+    int32_t reserved;
+    const double* cdf;       /* [S, A, B] p.cumsum(); cdf /= cdf[-1], as Generator.choice computes it (host numpy) */
+    const int32_t* next;     /* [S, A, B]                                                                       */
+    const double* reward;    /* [S, A]                                                                          */
+    const uint8_t* row_ok;   /* [S, A] 1 when Generator.choice accepts p[s, a] (no NaN, none negative, Kahan sum
+                                within sqrt(eps) of 1); sampling a row with 0 is the reference's ValueError       */
+} b2_finite_mdp_sampled;
+
 /* One decision step of n_envs HighwayLite states (15 physics sub-steps each).
  * Replaces `env.step(a)` on a deep-copied env: deterministic.py:36-43,
  * mcts.py:145,173.  states: [n_envs, 136] words, updated in place.
@@ -498,13 +512,12 @@ typedef struct b2_olop_tree {
 int b2_olop_plan(const b2_olop_config* cfg, const int32_t* root_states, const b2_olop_tree* tree,
                  uint64_t* rng, int8_t* plan, int32_t* result, void* stream);
 
-/* OLOP.plan on a finite MDP in any mode (b2_finite_mdp_sampled is declared with sparse sampling below).
+/* OLOP.plan on a finite MDP in any mode.
  * cfg->env_kind must be B2_ENV_FINITE; cfg->mdp is not read.  Every episode seeds the env copy's generator with
  * default_rng(np_random.randint(2**30)) (:73); with env_draws = 1 ("stochastic" / "sparse") each of the horizon
  * steps draws once from it (Generator.choice), after a terminal state too; with 0 (a "deterministic" table,
  * n_next = 1) none.  terminal: uint8 [n_states]; done = terminal[state before the step].  The tree is the same
  * open-loop tree as b2_olop_plan's; mu_ucb and upper differ from the host's only through CUDA's log. */
-struct b2_finite_mdp_sampled;
 int b2_olop_plan_sampled(const b2_olop_config* cfg, const struct b2_finite_mdp_sampled* mdp, const uint8_t* terminal,
                          int32_t env_draws, const int32_t* root_states, const b2_olop_tree* tree, uint64_t* rng,
                          int8_t* plan, int32_t* result, void* stream);
@@ -561,14 +574,13 @@ typedef struct b2_mdp_gape_tree {
 int b2_mdp_gape_plan(const b2_mdp_gape_config* cfg, const int32_t* root_states, const b2_mdp_gape_tree* tree,
                      uint64_t* rng, int8_t* plan, int32_t* result, void* stream);
 
-/* MDPGapE.plan on a finite MDP in any mode (b2_finite_mdp_sampled is declared with sparse sampling below).
+/* MDPGapE.plan on a finite MDP in any mode.
  * cfg->env_kind must be B2_ENV_FINITE; cfg->mdp is not read.  Every episode seeds the env copy's generator with
  * default_rng(np_random.randint(2**30)) (:67); with env_draws = 1 ("stochastic" / "sparse") every step draws once
  * from it (Generator.choice), with 0 (a "deterministic" table, n_next = 1) none.  terminal: uint8 [n_states]; done =
  * terminal[state before the step].  keys: int32 [n_trees, node_capacity], written: the state id a decision node was
  * observed under, -1 on unobserved placeholders, the root and chance nodes.  Floats are fp64 in the reference's order,
  * its dot products as fma chains; only CUDA's log / exp differ from the host's. */
-struct b2_finite_mdp_sampled;
 int b2_mdp_gape_plan_sampled(const b2_mdp_gape_config* cfg, const struct b2_finite_mdp_sampled* mdp,
                              const uint8_t* terminal, int32_t env_draws, const int32_t* root_states,
                              const b2_mdp_gape_tree* tree, int32_t* keys, uint64_t* rng, int8_t* plan, int32_t* result,
@@ -617,20 +629,6 @@ int b2_brue_plan(const b2_brue_config* cfg, const int32_t* root_states, const b2
  * env's `seed(np_random.randint(2**30))` and `Generator.choice(p.size, p=p)` replayed on the device) and HighwayLite.
  * The values are the reference's fp64 operations in its order: every node equals the reference's bit for bit.
  * ---------------------------------------------------------------------- */
-/* A finite MDP as the sampled env steps it (FiniteMDPEnv.step): r = reward[s, a]; k = searchsorted(cdf[s, a], u,
- * "right") for u = default_rng(seed).random(); s' = next[s, a, k]. */
-typedef struct b2_finite_mdp_sampled {
-    int32_t n_states;
-    int32_t n_actions;
-    int32_t n_next;          /* B: 1 "deterministic", S "stochastic" (next[s, a, k] = k), next's width "sparse" */
-    int32_t reserved;
-    const double* cdf;       /* [S, A, B] p.cumsum(); cdf /= cdf[-1], as Generator.choice computes it (host numpy) */
-    const int32_t* next;     /* [S, A, B]                                                                       */
-    const double* reward;    /* [S, A]                                                                          */
-    const uint8_t* row_ok;   /* [S, A] 1 when Generator.choice accepts p[s, a] (no NaN, none negative, Kahan sum
-                                within sqrt(eps) of 1); sampling a row with 0 is the reference's ValueError       */
-} b2_finite_mdp_sampled;
-
 typedef struct b2_sparse_sampling_config {
     int32_t env_kind;        /* B2_ENV_FINITE or B2_ENV_HIGHWAY                                                 */
     int32_t n_trees;

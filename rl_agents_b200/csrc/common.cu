@@ -43,6 +43,13 @@ int check_lane_env_il(int env_kind, int n_actions, const b2_finite_mdp& mdp) {
     }
     return check_lane_env(env_kind, n_actions, mdp);
 }
+
+int check_sampled_mdp(const b2_finite_mdp_sampled& mdp, int n_actions, const uint8_t* terminal, bool needs_terminal) {
+    B2_REQUIRE(mdp.cdf && mdp.next && mdp.reward && mdp.row_ok && (terminal || !needs_terminal),
+               "finite MDP tables missing");
+    B2_REQUIRE(mdp.n_actions == n_actions && mdp.n_states > 0 && mdp.n_next >= 1, "bad finite MDP shape");
+    return B2_OK;
+}
 }  // namespace b2
 
 extern "C" const char* b2_last_error(void) { return b2::g_err; }

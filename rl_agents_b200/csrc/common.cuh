@@ -37,6 +37,10 @@ int sm_count();
 int check_env_kind(int env_kind, int n_actions);
 int check_lane_env(int env_kind, int n_actions, const b2_finite_mdp& mdp);
 int check_lane_env_il(int env_kind, int n_actions, const b2_finite_mdp& mdp);
+// Launch check of a finite MDP stepped as FiniteMDPEnv.step (OLOP, MDP-GapE, MCTS-DPW, PlaTyPOOS, sparse sampling):
+// B2_OK, or B2_ERR_INVALID with the error set.  Its tables, and terminal when the planner reads it (needs_terminal),
+// then its shape against the planner's n_actions.
+int check_sampled_mdp(const b2_finite_mdp_sampled& mdp, int n_actions, const uint8_t* terminal, bool needs_terminal);
 
 // Blocks of 128 threads for n_trees trees of `group` lanes each.
 inline int lane_grid(int n_trees, int group) { return (n_trees * group + 127) / 128; }

@@ -1,14 +1,14 @@
-// Device env models of the one-tree-per-lane-group planners (mcts.cu, olop.cu, mdp_gape.cu, brue.cu): one tree per
-// lane on a finite MDP, one tree per 16-lane group on HighwayLite and IntersectionLite (lane = vehicle slot, the scene
-// in registers, so the reference's deep copy of the env is a register copy).  Each model reads only what it needs: the
-// finite tables, the root states and the action count.
+// Device env models of the one-tree-per-lane-group planners (mcts.cu, olop.cu, mdp_gape.cu, brue.cu, mcts_dpw.cu): one
+// tree per lane on a finite MDP, one tree per 16-lane group on HighwayLite and IntersectionLite (lane = vehicle slot, the
+// scene in registers, so the reference's deep copy of the env is a register copy).  Each model reads only what it
+// needs: the finite tables, the root states and the action count.
 //
 // step() reports truncation separately; MCTS reads it, the other planners pass a dummy (the reference's 4-tuple step
 // drops truncation).
 //
-// The planners that sample stochastic finite MDPs draw from a b2_finite_mdp_sampled row with searchsorted_right()
-// (sparse_sampling.cu, which seeds a fresh env generator per sample) or step it with sampled_next() (mcts_dpw.cu,
-// and SampledFiniteEnv in olop.cu and mdp_gape.cu).
+// A b2_finite_mdp_sampled row is sampled with sampled_next().  The planners that keep one env generator per episode
+// (olop.cu, mdp_gape.cu, mcts_dpw.cu) step SampledFiniteEnv with its step(); PlaTyPOOS (platypoos.cu) and sparse
+// sampling (sparse_sampling.cu) seed a fresh generator per child or sample and check row_ok in their own loops.
 #pragma once
 #include <type_traits>
 
@@ -38,20 +38,6 @@ __device__ __forceinline__ int sampled_next(const b2_finite_mdp_sampled& m, int6
     return m.next[row * B + k];
 }
 
-// A finite MDP in any mode, stepped as FiniteMDPEnv.step with the episode's env generator (env_rng).  It has no
-// step(): the planners step it in place with sampled_next(), after checking row_ok (kSampled<Env> selects that code).
-struct SampledFiniteEnv {
-    static constexpr int GROUP = 1;
-    int s;
-    Pcg64 env_rng;
-    __device__ __forceinline__ void load_root(const int32_t* root_states, int tree, int li) { s = root_states[tree]; }
-    __device__ __forceinline__ int avail(int n_actions, unsigned gmask) const { return (1 << n_actions) - 1; }
-    __device__ __forceinline__ static int nth(int mask, int n) { return n; }
-};
-
-template <class Env>
-constexpr bool kSampled = std::is_same<Env, SampledFiniteEnv>::value;
-
 struct FiniteEnv {
     static constexpr int GROUP = 1;
     int s;
@@ -69,6 +55,27 @@ struct FiniteEnv {
         return r;
     }
 };
+
+// A finite MDP in any mode, stepped as FiniteMDPEnv.step with the episode's env generator (env_rng; seeded by the
+// planner only when draw is set).  kSampled<Env> selects the code that calls this step().
+struct SampledFiniteEnv : FiniteEnv {
+    Pcg64 env_rng;
+    // FiniteMDPEnv.step on row s * n_actions + action.  With draw set, a row Generator.choice rejects (its ValueError)
+    // returns false with bad_row = the row and s unchanged.  Otherwise term = terminal[state BEFORE the transition],
+    // r = reward[row], and sampled_next() moves s.
+    __device__ __forceinline__ bool step(const b2_finite_mdp_sampled& m, const uint8_t* terminal, bool draw, int action,
+                                         bool& term, double& r, int& bad_row) {
+        const int64_t row = (int64_t)s * m.n_actions + action;
+        if (draw && !m.row_ok[row]) { bad_row = (int)row; return false; }
+        term = terminal[s] != 0;
+        r = m.reward[row];
+        s = sampled_next(m, row, draw, env_rng);
+        return true;
+    }
+};
+
+template <class Env>
+constexpr bool kSampled = std::is_same<Env, SampledFiniteEnv>::value;
 
 struct HighwayEnv {
     static constexpr int GROUP = 16;

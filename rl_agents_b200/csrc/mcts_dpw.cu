@@ -48,46 +48,27 @@ struct DpwArgs {
     int32_t* result;
 };
 
-// A finite MDP in any mode, stepped as FiniteMDPEnv.step with the run's env generator.
-struct DpwFinite {
-    static constexpr int GROUP = 1;
-    int s;
-    __device__ __forceinline__ void load_root(const int32_t* root_states, int tree, int li) { s = root_states[tree]; }
-    __device__ __forceinline__ int avail(int n_actions, unsigned gmask) const { return (1 << n_actions) - 1; }
-    __device__ __forceinline__ static int nth(int mask, int n) { return FiniteEnv::nth(mask, n); }
-    __device__ __forceinline__ static int rank_of(int mask, int action) { return FiniteEnv::rank_of(mask, action); }
-    __device__ __forceinline__ int obs_key(const b2_mcts_dpw_config& c) const { return c.obs_keys[s]; }
-    // -> the reward; bad_row >= 0: the row Generator.choice rejects (the state is left as it was)
-    __device__ __forceinline__ double step(const b2_mcts_dpw_config& c, int action, Pcg64& env_rng, int li,
-                                           unsigned gmask, bool& term, bool& trunc, int& bad_row) {
-        const b2_finite_mdp_sampled& m = c.mdp;
-        const int64_t row = (int64_t)s * m.n_actions + action;
-        if (c.env_draws && !m.row_ok[row]) { bad_row = (int)row; return 0.0; }
-        term = c.terminal[s] != 0;        // done = terminal[state BEFORE the transition]
+// Env::step on either model (the finite MDP with the run's env generator, HighwayLite deterministic); bad_row >= 0: the
+// finite row Generator.choice rejects
+template <class Env>
+__device__ __forceinline__ double dpw_step(Env& env, const b2_mcts_dpw_config& c, int action, int li, unsigned gmask,
+                                           bool& term, bool& trunc, int& bad_row) {
+    if constexpr (kSampled<Env>) {
+        double r = 0.0;
         trunc = false;
-        const double r = m.reward[row];
-        s = sampled_next(m, row, c.env_draws != 0, env_rng);
+        env.step(c.mdp, c.terminal, c.env_draws != 0, action, term, r, bad_row);
         return r;
+    } else {
+        return env.step(b2_finite_mdp{}, action, li, gmask, term, trunc);
     }
-};
+}
 
-struct DpwHighway {
-    static constexpr int GROUP = 16;
-    HighwayEnv e;
-    __device__ __forceinline__ void load_root(const int32_t* root_states, int tree, int li) {
-        e.load_root(root_states, tree, li);
-    }
-    __device__ __forceinline__ int avail(int n_actions, unsigned gmask) const { return e.avail(n_actions, gmask); }
-    __device__ __forceinline__ static int nth(int mask, int n) { return HighwayEnv::nth(mask, n); }
-    __device__ __forceinline__ static int rank_of(int mask, int action) { return HighwayEnv::rank_of(mask, action); }
-    // the observation is the step count t; the host turns it into sha1(str(t))[:5] for the dump.  The model is
-    // deterministic, so a chance node has one child either way.
-    __device__ __forceinline__ int obs_key(const b2_mcts_dpw_config& c) const { return e.t; }
-    __device__ __forceinline__ double step(const b2_mcts_dpw_config& c, int action, Pcg64& env_rng, int li,
-                                           unsigned gmask, bool& term, bool& trunc, int& bad_row) {
-        return e.step(b2_finite_mdp{}, action, li, gmask, term, trunc);
-    }
-};
+// The observation's key: the state's on the finite MDP; on HighwayLite the step count t, which the host turns into
+// sha1(str(t))[:5] for the dump (the model is deterministic, so a chance node has one child either way).
+template <class Env>
+__device__ __forceinline__ int obs_key(const Env& env, const b2_mcts_dpw_config& c) {
+    if constexpr (kSampled<Env>) return c.obs_keys[env.s]; else return env.t;
+}
 
 // DecisionNode / ChanceNode.__init__: value 0, count 0, appended to the parent's children after `last`
 __device__ __forceinline__ void new_node(const b2_mcts_dpw_tree& tr, int64_t nb, int id, int parent, int last,
@@ -125,8 +106,7 @@ __global__ void __launch_bounds__(128, Env::GROUP == 16 ? 4 : 8) mcts_dpw_kernel
         Env env;
         env.load_root(a.root_states, tree, li);                       // safe_deepcopy_env(state), mcts.py:183
         const uint32_t seed = rng.integers(1u << 30);                  // state.seed(np_random.randint(2**30)), :69
-        Pcg64 env_rng;
-        if (c.env_draws) env_rng.seed_from(seed);
+        if constexpr (kSampled<Env>) { if (c.env_draws) env.env_rng.seed_from(seed); }
         int node = 0, depth = 0;
         bool term = false, trunc = false;
         double total = 0.0;
@@ -168,11 +148,11 @@ __global__ void __launch_bounds__(128, Env::GROUP == 16 ? 4 : 8) mcts_dpw_kernel
                 }
                 action = tr.key[nb + chance];
             }
-            const double r = env.step(c, action, env_rng, li, gmask, term, trunc, bad_row);
+            const double r = dpw_step(env, c, action, li, gmask, term, trunc, bad_row);
             if (bad_row >= 0) { error = ERR_BAD_ROW; break; }
             ++steps;
             // ChanceNode.get_child (:171-182)
-            const int key = c.closed_loop ? env.obs_key(c) : c.open_key;
+            const int key = c.closed_loop ? obs_key(env, c) : c.open_key;
             int n_states = 0, lastk = -1, child = -1;
             for (int ch = tr.first_child[nb + chance]; ch >= 0; ch = tr.next_sibling[nb + ch]) {
                 if (tr.key[nb + ch] == key) { child = ch; break; }
@@ -210,7 +190,7 @@ __global__ void __launch_bounds__(128, Env::GROUP == 16 ? 4 : 8) mcts_dpw_kernel
                 for (int i = 0; i < n; ++i) idx += cdf[i] <= u ? 1 : 0;   // searchsorted(side='right')
                 idx = min(idx, n - 1);
                 const int action = c.rollout_policy != 1 ? Env::nth(pm, idx) : idx;
-                const double r = env.step(c, action, env_rng, li, gmask, term, trunc, bad_row);
+                const double r = dpw_step(env, c, action, li, gmask, term, trunc, bad_row);
                 if (bad_row >= 0) { error = ERR_BAD_ROW; break; }
                 ++steps;
                 total = total + c.gamma_pow[h] * r;
@@ -283,13 +263,11 @@ extern "C" int b2_mcts_dpw_plan(const b2_mcts_dpw_config* cfg, const int32_t* ro
     DpwArgs a;
     a.cfg = *cfg; a.tree = *tree; a.root_states = root_states; a.rng = rng; a.plan = plan; a.result = result;
     if (cfg->env_kind == B2_ENV_FINITE) {
-        const b2_finite_mdp_sampled& m = cfg->mdp;
-        B2_REQUIRE(m.cdf && m.next && m.reward && m.row_ok && cfg->terminal, "finite MDP tables missing");
+        if (check_sampled_mdp(cfg->mdp, cfg->n_actions, cfg->terminal, true) != B2_OK) return B2_ERR_INVALID;
         B2_REQUIRE(!cfg->closed_loop || cfg->obs_keys, "observation key table missing");
-        B2_REQUIRE(m.n_actions == cfg->n_actions && m.n_states > 0 && m.n_next >= 1, "bad finite MDP shape");
-        mcts_dpw_kernel<DpwFinite><<<lane_grid(cfg->n_trees, DpwFinite::GROUP), 128, 0, stream>>>(a);
+        mcts_dpw_kernel<SampledFiniteEnv><<<lane_grid(cfg->n_trees, SampledFiniteEnv::GROUP), 128, 0, stream>>>(a);
     } else {
-        mcts_dpw_kernel<DpwHighway><<<lane_grid(cfg->n_trees, DpwHighway::GROUP), 128, 0, stream>>>(a);
+        mcts_dpw_kernel<HighwayEnv><<<lane_grid(cfg->n_trees, HighwayEnv::GROUP), 128, 0, stream>>>(a);
     }
     B2_CUDA_CHECK(cudaGetLastError());
     return B2_OK;

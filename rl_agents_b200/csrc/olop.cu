@@ -115,22 +115,10 @@ __global__ void __launch_bounds__(128, 8) olop_kernel(OlopArgs a) {
             bool term, trunc;
             double r;                                                                   // olop.py:87
             if constexpr (kSampled<Env>) {
-                // FiniteMDPEnv.step: Generator.choice rejects the row (a ValueError), or done = terminal[state
-                // BEFORE the transition] and one draw of the env generator picks the next state
                 r = 0.0;
                 term = false;
-                if (live && !error) {
-                    const b2_finite_mdp_sampled& m = a.smdp;
-                    const int64_t row = (int64_t)env.s * m.n_actions + action;
-                    if (a.env_draws && !m.row_ok[row]) {
-                        error = ERR_BAD_ROW;
-                        bad_row = (int)row;
-                    } else {
-                        term = a.terminal[env.s] != 0;
-                        r = m.reward[row];
-                        env.s = sampled_next(m, row, a.env_draws != 0, env.env_rng);
-                    }
-                }
+                if (live && !error && !env.step(a.smdp, a.terminal, a.env_draws != 0, action, term, r, bad_row))
+                    error = ERR_BAD_ROW;
             } else {
                 r = env.step(a.cfg.mdp, action, li, gmask, term, trunc);
             }
@@ -234,8 +222,7 @@ extern "C" int b2_olop_plan_sampled(const b2_olop_config* cfg, const b2_finite_m
     B2_REQUIRE(cfg->env_kind == B2_ENV_FINITE, "env_kind must be B2_ENV_FINITE");
     B2_REQUIRE(cfg->n_trees > 0 && cfg->episodes >= 0 && cfg->horizon >= 1, "bad batch / budget");
     B2_REQUIRE(cfg->n_actions > 0 && cfg->n_actions <= 8, "n_actions must be in 1..8");
-    B2_REQUIRE(mdp->n_actions == cfg->n_actions && mdp->n_states > 0 && mdp->n_next > 0, "finite MDP shape");
-    B2_REQUIRE(mdp->cdf && mdp->next && mdp->reward && mdp->row_ok, "finite MDP tables missing");
+    if (check_sampled_mdp(*mdp, cfg->n_actions, terminal, true) != B2_OK) return B2_ERR_INVALID;
     B2_REQUIRE(env_draws == 0 || env_draws == 1, "env_draws must be 0 or 1");
     B2_REQUIRE((int64_t)cfg->node_capacity >= 1 + (int64_t)cfg->episodes * cfg->horizon * cfg->n_actions,
                "node_capacity too small");

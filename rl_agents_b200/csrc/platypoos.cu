@@ -422,9 +422,7 @@ extern "C" int b2_platypoos_plan(const b2_platypoos_config* cfg, const int32_t* 
     layout((char*)workspace, cfg->n_trees, cfg->layer_capacity, cfg->env_kind == B2_ENV_HIGHWAY, a.w);
     cudaStream_t stream = (cudaStream_t)stream_;
     if (cfg->env_kind == B2_ENV_FINITE) {
-        const b2_finite_mdp_sampled& m = cfg->mdp;
-        B2_REQUIRE(m.cdf && m.next && m.reward && m.row_ok && cfg->terminal, "finite MDP tables missing");
-        B2_REQUIRE(m.n_actions == cfg->n_actions && m.n_states > 0 && m.n_next >= 1, "bad finite MDP shape");
+        if (check_sampled_mdp(cfg->mdp, cfg->n_actions, cfg->terminal, true) != B2_OK) return B2_ERR_INVALID;
         platypoos_kernel<false><<<cfg->n_trees, THREADS, 0, stream>>>(a);
     } else {
         platypoos_kernel<true><<<cfg->n_trees, THREADS, 0, stream>>>(a);

@@ -317,9 +317,7 @@ extern "C" int b2_sparse_sampling_plan(const b2_sparse_sampling_config* cfg, con
     if (rc != B2_OK) return rc;
     cudaStream_t stream = (cudaStream_t)stream_;
     if (cfg->env_kind == B2_ENV_FINITE) {
-        const b2_finite_mdp_sampled& m = cfg->mdp;
-        B2_REQUIRE(m.cdf && m.next && m.reward && m.row_ok, "finite MDP tables missing");
-        B2_REQUIRE(m.n_actions == cfg->n_actions && m.n_states > 0 && m.n_next >= 1, "bad finite MDP shape");
+        if (check_sampled_mdp(cfg->mdp, cfg->n_actions, nullptr, false) != B2_OK) return B2_ERR_INVALID;
         layout((char*)workspace, cfg->n_trees, cfg->horizon, cfg->C, false, a.st);
         sparse_sampling_kernel<SFiniteEnv><<<lane_grid(cfg->n_trees, SFiniteEnv::GROUP), 128, 0, stream>>>(a);
     } else {

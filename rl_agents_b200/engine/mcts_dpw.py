@@ -99,10 +99,9 @@ class MCTSDPWEngine(TreeEngine):
         self.tables, self.terminal, self.obs_keys, env_draws, mdp_struct = None, None, None, 0, _lib.FiniteMDPSampled()
         if env_kind == _lib.ENV_FINITE:
             self.tables = SampledFiniteTables(mdp, self.device)
-            self.terminal = torch.as_tensor(np.ascontiguousarray(mdp.terminal, dtype=np.uint8), device=self.device)
+            self.terminal = self.tables.terminal
             self.obs_keys = torch.as_tensor(observation_keys(self.tables.n_states), device=self.device)
-            env_draws = int(mdp.mode != "deterministic")
-            mdp_struct = self.tables.struct()
+            env_draws, mdp_struct = self.tables.env_draws, self.tables.struct()
         self.cfg = _lib.MCTSDPWConfig(
             env_kind, self.n_trees, self.n_actions, self.episodes, self.horizon, self.capacity, rollout_id,
             rollout_action, int(self.closed_loop), OPEN_LOOP_KEY, env_draws, 0, float(temperature),
@@ -125,9 +124,7 @@ class MCTSDPWEngine(TreeEngine):
         err = res[:, 4]
         bad = np.nonzero(err == 2)[0]
         if bad.size:
-            p = self.tables.row(int(res[bad[0], 5]))
-            np.random.default_rng(0).choice(p.size, p=p)            # raises numpy's own message for this row
-            raise AssertionError("row %d was flagged but Generator.choice accepts it" % int(res[bad[0], 5]))
+            self.tables.raise_rejected_row(int(res[bad[0], 5]))
         if (err == 3).any():
             raise ValueError(EMPTY_ACTIONS_MESSAGE)
         if (err == 4).any():

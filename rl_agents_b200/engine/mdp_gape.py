@@ -51,7 +51,7 @@ class MDPGapEEngine(TreeEngine):
         self.tables, self.keys = None, None
         if self.sampled:
             self.tables = SampledFiniteTables(mdp, self.device)
-            self.terminal = torch.as_tensor(np.ascontiguousarray(mdp.terminal, dtype=np.uint8), device=self.device)
+            self.terminal = self.tables.terminal
             self.keys = torch.empty((self.n_trees, self.capacity), dtype=torch.int32, device=self.device)
         elif env_kind == _lib.ENV_FINITE:
             self.tables = FiniteTables(mdp, self.device)
@@ -68,7 +68,8 @@ class MDPGapEEngine(TreeEngine):
         self._load_rng(rng_words)
         if self.sampled:
             _lib.check(self.lib.b2_mdp_gape_plan_sampled(
-                self.cfg, self.tables.struct(), _lib.ptr(self.terminal), 1, _lib.ptr(root_states), self.tree,
+                self.cfg, self.tables.struct(), _lib.ptr(self.terminal), self.tables.env_draws,
+                _lib.ptr(root_states), self.tree,
                 _lib.ptr(self.keys), _lib.ptr(self.rng), _lib.ptr(self.plan_buf), _lib.ptr(self.result),
                 _lib.current_stream()))
             return
@@ -77,10 +78,8 @@ class MDPGapEEngine(TreeEngine):
 
     def _check(self, res):
         bad = np.nonzero(res[:, 2] == 4)[0]
-        if bad.size:                                  # a sampled row Generator.choice rejects: numpy's own message
-            p = self.tables.row(int(res[bad[0], 6]))
-            np.random.default_rng(0).choice(p.size, p=p)
-            raise AssertionError("row %d was flagged but Generator.choice accepts it" % int(res[bad[0], 6]))
+        if bad.size:
+            self.tables.raise_rejected_row(int(res[bad[0], 6]))
         if (res[:, 2] == 3).any():
             raise ValueError(PLACEHOLDERS_MESSAGE)                                   # mdp_gape.py:283-285
         if (res[:, 2] == 1).any():

@@ -114,9 +114,8 @@ class PlaTyPOOSEngine(TreeEngine):
         self.tables, self.terminal, env_draws, mdp_struct = None, None, 0, _lib.FiniteMDPSampled()
         if env_kind == _lib.ENV_FINITE:
             self.tables = SampledFiniteTables(mdp, self.device)
-            self.terminal = torch.as_tensor(np.ascontiguousarray(mdp.terminal, dtype=np.uint8), device=self.device)
-            env_draws = int(mdp.mode != "deterministic")
-            mdp_struct = self.tables.struct()
+            self.terminal = self.tables.terminal
+            env_draws, mdp_struct = self.tables.env_draws, self.tables.struct()
         self.cfg = _lib.PlaTyPOOSConfig(
             env_kind, self.n_trees, self.n_actions, self.horizon, self.node_capacity, self.layer_capacity, MAX_P,
             env_draws, self.p_top.data_ptr(), self.nodes_count.data_ptr(), self.evaluations.data_ptr(),
@@ -141,9 +140,7 @@ class PlaTyPOOSEngine(TreeEngine):
         err = res[:, 3]
         bad = np.nonzero(err == 2)[0]
         if bad.size:
-            p = self.tables.row(int(res[bad[0], 4]))
-            np.random.default_rng(0).choice(p.size, p=p)            # raises numpy's own message for this row
-            raise AssertionError("row %d was flagged but Generator.choice accepts it" % int(res[bad[0], 4]))
+            self.tables.raise_rejected_row(int(res[bad[0], 4]))
         if (err == 4).any():
             raise ValueError(EMPTY_CANDIDATES_MESSAGE)
         if (err == 3).any():

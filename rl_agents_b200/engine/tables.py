@@ -97,7 +97,9 @@ def sampled_mdp_tables(mdp):
 
 
 class SampledFiniteTables(object):
-    """Device copy of a finite MDP in any mode, for the planners that sample transitions (sparse sampling)."""
+    """Device copy of a finite MDP in any mode, stepped as FiniteMDPEnv.step by the planners that sample transitions
+    (OLOP, MDP-GapE, MCTS-DPW, PlaTyPOOS, sparse sampling): the b2_finite_mdp_sampled tables, terminal (uint8 [S],
+    done = terminal[state before the step]) and env_draws (1 when a step draws from the env's generator)."""
 
     def __init__(self, mdp, device):
         import torch
@@ -107,10 +109,15 @@ class SampledFiniteTables(object):
         self.n_states, self.n_actions, self.n_next = t["cdf"].shape
         for k, v in t.items():
             setattr(self, k, torch.as_tensor(v, device=device))
+        self.terminal = torch.as_tensor(np.ascontiguousarray(mdp.terminal, dtype=np.uint8), device=device)
+        self.env_draws = int(mdp.mode != "deterministic")
 
-    def row(self, row):
-        """The probability row s * A + a, as Generator.choice reads it."""
-        return self.p.reshape(-1, self.p.shape[-1])[row]
+    def raise_rejected_row(self, row):
+        """Raise what Generator.choice raises on the probability row s * A + a that a kernel flagged (numpy's own
+        ValueError, as the reference's env step does), or AssertionError if numpy accepts it."""
+        p = self.p.reshape(-1, self.p.shape[-1])[row]
+        np.random.default_rng(0).choice(p.size, p=p)
+        raise AssertionError("row %d was flagged but Generator.choice accepts it" % row)
 
     def struct(self):
         from rl_agents_b200 import _lib
