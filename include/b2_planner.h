@@ -423,7 +423,10 @@ typedef struct b2_mcts_tree {
 
 #define B2_PCG64_STATE_WORDS 6 /* uint64: state hi,lo, inc hi,lo, has_uint32, uinteger */
 #define B2_MCTS_RESULT_WORDS 8
-/* per tree int32 result: [0] n_nodes [1] plan_len [2] env steps taken */
+/* per tree int32 result: [0] n_nodes [1] plan_len [2] env steps taken
+ * [3] b2_mcts_plan_sampled: error (1: a reached probability row that Generator.choice rejects)
+ * [4] b2_mcts_plan_sampled: that row s * n_actions + a, else -1.  [3] and [4] are not written by b2_mcts_plan.
+ *     An error stops its own tree only. */
 
 /* MCTS.plan (:179-184) for n_trees independent decisions, strict episode order
  * inside each tree, consuming each tree's numpy PCG64 stream exactly as
@@ -432,6 +435,17 @@ typedef struct b2_mcts_tree {
  * env_kind: B2_ENV_FINITE, B2_ENV_HIGHWAY (5 actions) or B2_ENV_INTERSECTION (3 actions). */
 int b2_mcts_plan(const b2_mcts_config* cfg, const int32_t* root_states, const b2_mcts_tree* tree,
                  uint64_t* rng, int8_t* plan, int32_t* result, void* stream);
+
+/* MCTS.plan on a finite MDP in any mode.
+ * cfg->env_kind must be B2_ENV_FINITE; cfg->mdp is not read.  The reference never reseeds its env copies, so every
+ * episode's deep copy (:183) starts from the live env's generator: env_rng, uint64 [n_trees, 6] in the layout of rng,
+ * read only.  With env_draws = 1 ("stochastic" / "sparse") every step an episode takes, selection or rollout, draws
+ * once from that copy (Generator.choice), so step k of every episode uses the k-th double of the same stream; with
+ * 0 (a "deterministic" table, n_next = 1) none.  terminal: uint8 [n_states]; done = terminal[state before the step].
+ * The tree is the same open-loop tree as b2_mcts_plan's; resume_nodes ("subtree") works as there. */
+int b2_mcts_plan_sampled(const b2_mcts_config* cfg, const struct b2_finite_mdp_sampled* mdp, const uint8_t* terminal,
+                         int32_t env_draws, const uint64_t* env_rng, const int32_t* root_states,
+                         const b2_mcts_tree* tree, uint64_t* rng, int8_t* plan, int32_t* result, void* stream);
 
 /* ------------------------------------------------------------------------
  * Wavefront MCTS: ONE decision searched by the whole GPU.  The reference's episode (selection mcts.py:141-149,
@@ -470,6 +484,17 @@ int64_t b2_mcts_wave_workspace_bytes(const b2_mcts_wave_config* cfg);
  * [0] node_capacity [1] plan_len [2] env steps [3] waves [4..7] phase clocks.  Cooperative launch. */
 int b2_mcts_plan_wave(const b2_mcts_wave_config* cfg, const int32_t* root_state, const b2_mcts_wave_tree* tree,
                       void* workspace, int8_t* plan, int32_t* result, void* stream);
+
+/* b2_mcts_plan_wave on a finite MDP in any mode.
+ * cfg->env_kind must be B2_ENV_FINITE; cfg->mdp is not read.  mdp, terminal and env_draws as in b2_mcts_plan_sampled;
+ * env_rng: uint64 [6], the live env's generator, which every episode's env copy starts from, so step h of every
+ * episode draws the same double of its stream.  rejected: int32 [2], the lowest episode that reaches a probability
+ * row Generator.choice rejects and that row s * n_actions + a, else -1 -1; the search stops after that episode's
+ * wave.  result as for b2_mcts_plan_wave. */
+int b2_mcts_plan_wave_sampled(const b2_mcts_wave_config* cfg, const struct b2_finite_mdp_sampled* mdp,
+                              const uint8_t* terminal, int32_t env_draws, const uint64_t* env_rng,
+                              const int32_t* root_state, const b2_mcts_wave_tree* tree, void* workspace, int8_t* plan,
+                              int32_t* result, int32_t* rejected, void* stream);
 
 /* ------------------------------------------------------------------------
  * OLOP / KL-OLOP -- rl_agents/agents/tree_search/olop.py

@@ -254,9 +254,13 @@ EXPORTS = {
     "b2_opd_copy_tree": (c_int, [c_void_p, c_int32, c_int32] + [c_void_p] * 7),
     "b2_mcts_plan": (c_int, [ctypes.POINTER(MCTSConfig), c_void_p, ctypes.POINTER(MCTSTree), c_void_p, c_void_p,
                              c_void_p, c_void_p]),
+    "b2_mcts_plan_sampled": (c_int, [ctypes.POINTER(MCTSConfig), ctypes.POINTER(FiniteMDPSampled), c_void_p, c_int32,
+                                     c_void_p, c_void_p, ctypes.POINTER(MCTSTree)] + [c_void_p] * 4),
     "b2_mcts_wave_workspace_bytes": (c_int64, [ctypes.POINTER(MCTSWaveConfig)]),
     "b2_mcts_plan_wave": (c_int, [ctypes.POINTER(MCTSWaveConfig), c_void_p, ctypes.POINTER(MCTSWaveTree), c_void_p,
                                   c_void_p, c_void_p, c_void_p]),
+    "b2_mcts_plan_wave_sampled": (c_int, [ctypes.POINTER(MCTSWaveConfig), ctypes.POINTER(FiniteMDPSampled), c_void_p,
+                                          c_int32, c_void_p, c_void_p, ctypes.POINTER(MCTSWaveTree)] + [c_void_p] * 5),
     "b2_olop_plan": (c_int, [ctypes.POINTER(OLOPConfig), c_void_p, ctypes.POINTER(OLOPTree), c_void_p, c_void_p,
                              c_void_p, c_void_p]),
     "b2_olop_plan_sampled": (c_int, [ctypes.POINTER(OLOPConfig), ctypes.POINTER(FiniteMDPSampled), c_void_p, c_int32,

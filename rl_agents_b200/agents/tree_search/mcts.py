@@ -32,11 +32,14 @@ class MCTS(AbstractPlanner):
         self.rollout_policy = rollout_policy
         if not self.config["horizon"]:                                   # mcts.py:116-118
             self.config["episodes"], self.config["horizon"] = allocation(self.config["budget"], self.config["gamma"])
-        # closed_loop (mcts.py:125,147,267-273) keys an extra node level on str(observation).  The device env
-        # models (finite MDPs, HighwayLite, IntersectionLite) are deterministic: every action node then has exactly one observation child carrying the same
-        # statistics, so visit counts, values and the recommended action equal the open-loop search's
-        # (golden: tests/golden "mcts_closed_loop", produced by the reference with closed_loop=True).  The
-        # reference's get_plan interleaves the observation keys with the actions; here the plan lists actions.
+        # closed_loop (mcts.py:125,147,267-273) keys an extra node level on str(observation).  Within one plan() the
+        # successor after a given action prefix is fixed: HighwayLite, IntersectionLite and deterministic finite MDPs
+        # are deterministic, and the env copies of a stochastic finite MDP all replay the live env's generator (the
+        # reference never reseeds them).  Every action node then has exactly one observation child carrying the same
+        # statistics, so visit counts, values and the recommended action equal the open-loop search's (goldens:
+        # tests/golden "mcts_closed_loop" and golden_mcts_stochastic.json, produced by the reference with
+        # closed_loop=True).  The reference's get_plan interleaves the observation keys with the actions; here the
+        # plan lists actions.
 
     @classmethod
     def default_config(cls):
@@ -83,7 +86,7 @@ class MCTS(AbstractPlanner):
     def plan(self, state, observation):
         import torch
         from rl_agents_b200.engine.mcts import pcg64_words
-        d = describe(state)
+        d = describe(state, env_words=True)
         replicas = int(self.config.get("root_parallel", 1) or 1)
         root = torch.from_numpy(d.root.reshape(1, -1) if d.root.size > 1 else d.root)
         width = int(self.config.get("wavefront", 0) or 0)
@@ -100,7 +103,7 @@ class MCTS(AbstractPlanner):
                                                                  self.config["horizon"], self.config["gamma"],
                                                                  self.config["temperature"], width, mdp=d.mdp))
             seed = int(self.np_random.integers(0, 2 ** 63 - 1))
-            eng.plan(root.reshape(-1).to(eng.device).contiguous(), seed)
+            eng.plan(root.reshape(-1).to(eng.device).contiguous(), seed, d.env_words)
             plan, _ = eng.finish()
             self.last_tree = eng
             counts, values = eng.root_statistics()
@@ -110,7 +113,7 @@ class MCTS(AbstractPlanner):
             # the reference's semantics: one tree, strict episode order, the planner's own RNG stream
             eng = self._engine_for(d, 1, self.config["episodes"])
             resume = [self._resume] if getattr(self, "_resume", 0) > 0 else None
-            plan, _ = self.search_one_tree(eng, d, resume)
+            plan, _ = self.search_one_tree(eng, d, resume, d.env_words)
             self._resume = 0
             return plan
         # extension ("root_parallel": R): R independent trees of episodes/R episodes from the same root,
@@ -120,7 +123,8 @@ class MCTS(AbstractPlanner):
         eng = self._engine_for(d, replicas, episodes)
         gens = self.np_random.spawn(replicas)
         roots = root.repeat(replicas, 1) if d.root.size > 1 else root.repeat(replicas)
-        eng.plan(roots.to(eng.device).contiguous(), np.stack([pcg64_words(g) for g in gens]))
+        # every replica copies the same env, so every replica's env copies start from the same generator words
+        eng.plan(roots.to(eng.device).contiguous(), np.stack([pcg64_words(g) for g in gens]), None, d.env_words)
         plans, res, _ = eng.finish()
         self.last_tree = eng
         fc = eng.first_child[:, 0].cpu().numpy()

@@ -9,6 +9,11 @@
 // scene lives in registers and is "deep-copied" from the root once per episode,
 // mcts.py:183), 1 lane for finite MDPs.  Tree bookkeeping is group-uniform
 // scalar code; lane 0 of the group performs the stores.
+//
+// SampledFiniteEnv (b2_mcts_plan_sampled) steps a finite MDP in any mode as FiniteMDPEnv.step does.  The reference
+// never reseeds its env copies, so every episode's deep copy starts from the live env's generator: each episode loads
+// the tree's env words, and step k of every episode draws the k-th double of that one stream.  Only the steps the
+// reference takes draw or check a row; a reached row Generator.choice rejects stops its own tree.
 #include "common.cuh"
 #include "lane_env.cuh"
 #include "pcg64.cuh"
@@ -16,6 +21,7 @@
 namespace b2 {
 
 constexpr int MAX_BRANCH_MCTS = 8;
+constexpr int ERR_BAD_ROW = 1;
 
 struct MctsArgs {
     b2_mcts_config cfg;
@@ -24,6 +30,11 @@ struct MctsArgs {
     uint64_t* rng;
     int8_t* plan;
     int32_t* result;
+    // SampledFiniteEnv only
+    b2_finite_mdp_sampled smdp;
+    const uint8_t* terminal;
+    int32_t env_draws;
+    const uint64_t* env_rng;
 };
 
 // --------------------------------------------------------------- kernel ---
@@ -53,10 +64,13 @@ __global__ void __launch_bounds__(128, B2_MCTS_MIN_BLOCKS) mcts_kernel(MctsArgs 
     }
     __syncwarp(gmask);
     int n_nodes = resume > 0 ? resume : 1, env_steps = 0;   // resume: a re-rooted sub-tree is already in place
+    int error = 0, bad_row = -1;
 
     for (int ep = 0; ep < a.cfg.episodes; ++ep) {
+        if constexpr (kSampled<Env>) { if (error) break; }
         Env env;
         env.load_root(a.root_states, tree, li);     // safe_deepcopy_env(state), mcts.py:183
+        if constexpr (kSampled<Env>) env.env_rng.load(a.env_rng + (int64_t)tree * B2_PCG64_STATE_WORDS);
         int node = 0;
         bool in_sel = true, active = live;
         double total = 0.0;
@@ -136,7 +150,17 @@ __global__ void __launch_bounds__(128, B2_MCTS_MIN_BLOCKS) mcts_kernel(MctsArgs 
             }
             bool term, trunc;
             Env next = env;
-            const double r = next.step(a.cfg.mdp, action, li, gmask, term, trunc);
+            double r;
+            if constexpr (kSampled<Env>) {
+                // only a step the reference takes draws or checks its row
+                r = 0.0; term = false; trunc = false;
+                if (active && !next.step(a.smdp, a.terminal, a.env_draws != 0, action, term, r, bad_row)) {
+                    error = ERR_BAD_ROW;
+                    active = false;
+                }
+            } else {
+                r = next.step(a.cfg.mdp, action, li, gmask, term, trunc);
+            }
             if (active) {
                 env = next;
                 ++env_steps;
@@ -150,7 +174,7 @@ __global__ void __launch_bounds__(128, B2_MCTS_MIN_BLOCKS) mcts_kernel(MctsArgs 
             }
         }
         // update_branch (mcts.py:257-265)
-        if (writer) {
+        if (writer && !error) {
             int n = node;
             while (n >= 0) {
                 const int c = tr.count[nb + n] + 1;
@@ -184,6 +208,7 @@ __global__ void __launch_bounds__(128, B2_MCTS_MIN_BLOCKS) mcts_kernel(MctsArgs 
         res[0] = n_nodes;
         res[1] = len;
         res[2] = env_steps;
+        if constexpr (kSampled<Env>) { res[3] = error; res[4] = bad_row; }
     }
 }
 
@@ -191,9 +216,7 @@ __global__ void __launch_bounds__(128, B2_MCTS_MIN_BLOCKS) mcts_kernel(MctsArgs 
 
 using namespace b2;
 
-extern "C" int b2_mcts_plan(const b2_mcts_config* cfg, const int32_t* root_states, const b2_mcts_tree* tree,
-                            uint64_t* rng, int8_t* plan, int32_t* result, void* stream_) {
-    B2_REQUIRE(cfg && root_states && tree && rng && plan && result, "null pointer");
+static int check_mcts_config(const b2_mcts_config* cfg) {
     B2_REQUIRE(cfg->n_trees > 0 && cfg->episodes >= 0 && cfg->horizon >= 0, "bad batch / budget");
     B2_REQUIRE(cfg->n_actions > 0 && cfg->n_actions <= MAX_BRANCH_MCTS, "n_actions must be in 1..8");
     B2_REQUIRE((int64_t)cfg->node_capacity >= 1 + (int64_t)cfg->episodes * cfg->n_actions, "node_capacity too small");
@@ -202,6 +225,13 @@ extern "C" int b2_mcts_plan(const b2_mcts_config* cfg, const int32_t* root_state
                "policy must be 0 (random_available), 1 (random) or 2 (preference)");
     B2_REQUIRE((cfg->prior_policy != 2 || cfg->pref_prior) && (cfg->rollout_policy != 2 || cfg->pref_cdf),
                "preference policy tables missing");
+    return B2_OK;
+}
+
+extern "C" int b2_mcts_plan(const b2_mcts_config* cfg, const int32_t* root_states, const b2_mcts_tree* tree,
+                            uint64_t* rng, int8_t* plan, int32_t* result, void* stream_) {
+    B2_REQUIRE(cfg && root_states && tree && rng && plan && result, "null pointer");
+    if (check_mcts_config(cfg) != B2_OK) return B2_ERR_INVALID;
     const int rc = check_lane_env_il(cfg->env_kind, cfg->n_actions, cfg->mdp);
     if (rc != B2_OK) return rc;
     cudaStream_t stream = (cudaStream_t)stream_;
@@ -213,6 +243,24 @@ extern "C" int b2_mcts_plan(const b2_mcts_config* cfg, const int32_t* root_state
         mcts_kernel<HighwayEnv><<<lane_grid(cfg->n_trees, HighwayEnv::GROUP), 128, 0, stream>>>(a);
     else
         mcts_kernel<IntersectionEnv><<<lane_grid(cfg->n_trees, IntersectionEnv::GROUP), 128, 0, stream>>>(a);
+    B2_CUDA_CHECK(cudaGetLastError());
+    return B2_OK;
+}
+
+extern "C" int b2_mcts_plan_sampled(const b2_mcts_config* cfg, const b2_finite_mdp_sampled* mdp, const uint8_t* terminal,
+                                    int32_t env_draws, const uint64_t* env_rng, const int32_t* root_states,
+                                    const b2_mcts_tree* tree, uint64_t* rng, int8_t* plan, int32_t* result,
+                                    void* stream_) {
+    B2_REQUIRE(cfg && mdp && env_rng && root_states && tree && rng && plan && result, "null pointer");
+    B2_REQUIRE(cfg->env_kind == B2_ENV_FINITE, "env_kind must be B2_ENV_FINITE");
+    if (check_mcts_config(cfg) != B2_OK) return B2_ERR_INVALID;
+    if (check_sampled_mdp(*mdp, cfg->n_actions, terminal, true) != B2_OK) return B2_ERR_INVALID;
+    B2_REQUIRE(env_draws == 0 || env_draws == 1, "env_draws must be 0 or 1");
+    cudaStream_t stream = (cudaStream_t)stream_;
+    MctsArgs a;
+    a.cfg = *cfg; a.tree = *tree; a.root_states = root_states; a.rng = rng; a.plan = plan; a.result = result;
+    a.smdp = *mdp; a.terminal = terminal; a.env_draws = env_draws; a.env_rng = env_rng;
+    mcts_kernel<SampledFiniteEnv><<<lane_grid(cfg->n_trees, SampledFiniteEnv::GROUP), 128, 0, stream>>>(a);
     B2_CUDA_CHECK(cudaGetLastError());
     return B2_OK;
 }

@@ -14,8 +14,16 @@
 //                    rollout to the horizon; then count += 1, value_sum += return along the path with integer
 //                    atomics on a 2^-40 fixed-point sum (order independent, exact).
 // Specification: oracle/planners.py::mcts_plan_wavefront (bit-identical: node ids, counts, value sums).
+//
+// b2_mcts_plan_wave_sampled runs a finite MDP in any mode (mcts_wave_kernel<true>).  Every episode's env is a deep
+// copy of the same live env, generator included, so step h of every episode draws the same double u[h] of that
+// generator's stream: each CTA computes the horizon's doubles once and a step is searchsorted(cdf[row], u[h]).  The
+// lowest episode that reaches a row Generator.choice rejects is reported (that episode backs nothing up), and the
+// search stops after its wave.
 #include "common.cuh"
 #include "highway_lite.cuh"
+#include "lane_env.cuh"
+#include "pcg64.cuh"
 
 namespace b2 {
 namespace mwave {
@@ -31,6 +39,7 @@ struct Control {
     unsigned bar_count, bar_gen;
     int env_steps, pad;
     long long prof[4];       // CTA 0 clock64 totals: 0 select, 1 barrier, 2 simulate, 3 barrier
+    unsigned long long rejected;   // sampled: max of ~(episode << 32 | row) over the rejected rows reached; 0 none
 };
 
 struct Args {
@@ -44,6 +53,12 @@ struct Args {
     double* recip;           // [episodes + width + 2] 1.0 / k (filled at kernel start)
     int8_t* plan;
     int32_t* result;
+    // mcts_wave_kernel<true> only
+    b2_finite_mdp_sampled smdp;
+    const uint8_t* terminal;
+    int32_t env_draws;
+    const uint64_t* env_rng;
+    int32_t* rejected;       // [2] episode, row
 };
 
 __device__ __forceinline__ unsigned long long splitmix64(unsigned long long x) {
@@ -276,6 +291,22 @@ __device__ __forceinline__ void backup(const Args& a, int j, int reached, double
     }
 }
 
+// FiniteMDPEnv.step of a sampled table at step h of an episode (u: the env stream's doubles); false with `row` set
+// when the row is one Generator.choice rejects
+__device__ __forceinline__ bool sampled_step(const Args& a, const double* u, int h, int& s, int action, double& r,
+                                             bool& term, int& row) {
+    const b2_finite_mdp_sampled& m = a.smdp;
+    const int64_t rw = (int64_t)s * m.n_actions + action;
+    if (a.env_draws && !m.row_ok[rw]) { row = (int)rw; return false; }
+    term = a.terminal[s] != 0;
+    r = m.reward[rw];
+    const int B = m.n_next;
+    const int k = a.env_draws ? searchsorted_right(m.cdf + rw * B, B, u[h]) : 0;
+    s = m.next[rw * B + k];
+    return true;
+}
+
+template <bool SAMPLED>
 __global__ void __launch_bounds__(THREADS, 1) mcts_wave_kernel(Args a) {
     extern __shared__ long long score_table[];
     __shared__ SelShared sh;
@@ -283,7 +314,18 @@ __global__ void __launch_bounds__(THREADS, 1) mcts_wave_kernel(Args a) {
     const unsigned n_ctas = gridDim.x;
     Control* ctl = a.ctl;
     const b2_mcts_wave_tree& tr = a.tree;
-    const bool hwy = a.cfg.env_kind == B2_ENV_HIGHWAY;
+    const bool hwy = !SAMPLED && a.cfg.env_kind == B2_ENV_HIGHWAY;
+    const double* env_u = nullptr;
+    if constexpr (SAMPLED) {
+        // the env copies' common stream: step h of every episode draws env_u[h]
+        __shared__ double u_sh[MAX_H];
+        if (tid == 0 && a.env_draws) {
+            Pcg64 g;
+            g.load(a.env_rng);
+            for (int h = 0; h < a.cfg.horizon; ++h) u_sh[h] = g.random();
+        }
+        env_u = u_sh;
+    }
     const int A = a.cfg.n_actions, H = a.cfg.horizon, E = a.cfg.episodes, W = a.cfg.width;
     // node arrays: root + unused marks (parent -2); every CTA clears a slice
     for (int i = blockIdx.x * THREADS + tid; i < a.cfg.node_capacity; i += THREADS * (int)n_ctas) {
@@ -376,19 +418,25 @@ __global__ void __launch_bounds__(THREADS, 1) mcts_wave_kernel(Args a) {
                 int s = a.root_state[0];
                 double total = 0.0;
                 bool terminal = false;
-                int reached = 0;
+                int reached = 0, bad_row = -1;
                 for (int h = 0; h < depth; ++h) {
                     const int node = __ldcg(a.paths + (int64_t)j * H + h);
                     const int action = __ldcg(tr.meta + node) & 0xff;
-                    const double r = m.reward[(int64_t)s * m.n_actions + action];
-                    const bool term = m.terminal[s] != 0;
-                    s = m.transition[(int64_t)s * m.n_actions + action];
+                    double r;
+                    bool term;
+                    if constexpr (SAMPLED) {
+                        if (!sampled_step(a, env_u, h, s, action, r, term, bad_row)) break;
+                    } else {
+                        r = m.reward[(int64_t)s * m.n_actions + action];
+                        term = m.terminal[s] != 0;
+                        s = m.transition[(int64_t)s * m.n_actions + action];
+                    }
                     ++env_steps;
                     total += a.cfg.gamma_pow[h] * r;
                     reached = h + 1;
                     if (term) { terminal = true; break; }
                 }
-                if (!terminal) {
+                if (!terminal && bad_row < 0) {
                     if (depth < H && __ldcg(a.expands + j)) {
                         const int leaf = depth > 0 ? __ldcg(a.paths + (int64_t)j * H + depth - 1) : 0;
                         const int base = 1 + e * A;
@@ -398,20 +446,32 @@ __global__ void __launch_bounds__(THREADS, 1) mcts_wave_kernel(Args a) {
                     }
                     for (int h = depth; h < H; ++h) {
                         const int action = wave_random(a.cfg.seed, e, h, 1, A);
-                        const double r = m.reward[(int64_t)s * m.n_actions + action];
-                        const bool term = m.terminal[s] != 0;
-                        s = m.transition[(int64_t)s * m.n_actions + action];
+                        double r;
+                        bool term;
+                        if constexpr (SAMPLED) {
+                            if (!sampled_step(a, env_u, h, s, action, r, term, bad_row)) break;
+                        } else {
+                            r = m.reward[(int64_t)s * m.n_actions + action];
+                            term = m.terminal[s] != 0;
+                            s = m.transition[(int64_t)s * m.n_actions + action];
+                        }
                         ++env_steps;
                         total += a.cfg.gamma_pow[h] * r;
                         if (term) break;
                     }
                 }
-                backup(a, j, reached, total, 0, 1, 0u);
+                if (SAMPLED && bad_row >= 0)
+                    atomicMax(&ctl->rejected, ~(((unsigned long long)e << 32) | (unsigned)bad_row));
+                else
+                    backup(a, j, reached, total, 0, 1, 0u);
             }
         }
         lap(2);
         grid_barrier(ctl, n_ctas);
         lap(3);
+        if constexpr (SAMPLED) {
+            if (*(volatile unsigned long long*)&ctl->rejected) break;    // the reference raises in this wave
+        }
     }
     // env steps: one count per episode (lane 0 of writer groups / finite threads)
     if (hwy) {
@@ -446,6 +506,11 @@ __global__ void __launch_bounds__(THREADS, 1) mcts_wave_kernel(Args a) {
         a.result[2] = *(volatile int*)&ctl->env_steps;
         a.result[3] = (E + W - 1) / W;
         for (int i = 0; i < 4; ++i) a.result[4 + i] = (int32_t)(ctl->prof[i] >> 8);
+        if constexpr (SAMPLED) {
+            const unsigned long long k = ~*(volatile unsigned long long*)&ctl->rejected;
+            a.rejected[0] = ~k ? (int32_t)(k >> 32) : -1;
+            a.rejected[1] = ~k ? (int32_t)(unsigned)k : -1;
+        }
     }
 }
 
@@ -472,15 +537,46 @@ extern "C" int64_t b2_mcts_wave_workspace_bytes(const b2_mcts_wave_config* cfg) 
     return mwave::make_layout(cfg).total;
 }
 
-extern "C" int b2_mcts_plan_wave(const b2_mcts_wave_config* cfg, const int32_t* root_state, const b2_mcts_wave_tree* tree,
-                                 void* workspace, int8_t* plan, int32_t* result, void* stream_) {
-    B2_REQUIRE(cfg && root_state && tree && workspace && plan && result, "null pointer");
+static int check_wave_config(const b2_mcts_wave_config* cfg) {
     B2_REQUIRE(cfg->episodes >= 0 && cfg->horizon >= 0 && cfg->horizon <= mwave::MAX_H, "bad budget / horizon (<= 64)");
     B2_REQUIRE(cfg->width >= 1 && cfg->width <= mwave::MAX_WIDTH, "wave width must be in 1..1024");
     B2_REQUIRE(cfg->n_actions > 0 && cfg->n_actions <= mwave::MAX_A, "n_actions must be in 1..8");
     B2_REQUIRE((int64_t)cfg->node_capacity >= 1 + (int64_t)cfg->episodes * cfg->n_actions, "node_capacity too small");
     B2_REQUIRE(cfg->gamma_pow, "gamma table missing");
     B2_REQUIRE(cfg->rollout_policy == 0 && cfg->prior_policy == 0, "wavefront MCTS implements the random_available policies");
+    return B2_OK;
+}
+
+// the workspace carve-up and the cooperative launch of mcts_wave_kernel<SAMPLED> on the filled-in Args
+template <bool SAMPLED>
+static int launch_wave(const b2_mcts_wave_config* cfg, mwave::Args& a, void* workspace, cudaStream_t stream) {
+    const mwave::Layout l = mwave::make_layout(cfg);
+    char* ws = (char*)workspace;
+    a.ctl = (mwave::Control*)(ws + l.ctl);
+    a.paths = (int32_t*)(ws + l.paths);
+    a.plen = (int32_t*)(ws + l.plen);
+    a.expands = (int32_t*)(ws + l.expands);
+    a.recip = (double*)(ws + l.recip);
+    B2_CUDA_CHECK(cudaMemsetAsync(a.ctl, 0, sizeof(mwave::Control), stream));
+    const size_t smem = (size_t)mwave::TABLE_KEYS * 8;
+    B2_CUDA_CHECK(cudaFuncSetAttribute(mwave::mcts_wave_kernel<SAMPLED>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)smem));
+    int per_sm = 0;
+    B2_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, mwave::mcts_wave_kernel<SAMPLED>,
+                                                                mwave::THREADS, smem));
+    B2_REQUIRE(per_sm >= 1, "wave kernel does not fit on an SM");
+    int grid = sm_count();
+    if (cfg->max_ctas > 0 && cfg->max_ctas < grid) grid = cfg->max_ctas;
+    void* params[] = {&a};
+    B2_CUDA_CHECK(cudaLaunchCooperativeKernel((const void*)mwave::mcts_wave_kernel<SAMPLED>, dim3(grid),
+                                              dim3(mwave::THREADS), params, smem, stream));
+    return B2_OK;
+}
+
+extern "C" int b2_mcts_plan_wave(const b2_mcts_wave_config* cfg, const int32_t* root_state, const b2_mcts_wave_tree* tree,
+                                 void* workspace, int8_t* plan, int32_t* result, void* stream_) {
+    B2_REQUIRE(cfg && root_state && tree && workspace && plan && result, "null pointer");
+    if (check_wave_config(cfg) != B2_OK) return B2_ERR_INVALID;
     if (cfg->env_kind == B2_ENV_FINITE) {
         B2_REQUIRE(cfg->mdp.transition && cfg->mdp.reward && cfg->mdp.terminal, "finite MDP tables missing");
         B2_REQUIRE(cfg->mdp.n_actions == cfg->n_actions, "mdp.n_actions != n_actions");
@@ -490,27 +586,24 @@ extern "C" int b2_mcts_plan_wave(const b2_mcts_wave_config* cfg, const int32_t* 
         set_error("unknown env_kind %d", cfg->env_kind);
         return B2_ERR_INVALID;
     }
-    cudaStream_t stream = (cudaStream_t)stream_;
-    const mwave::Layout l = mwave::make_layout(cfg);
-    char* ws = (char*)workspace;
     mwave::Args a;
     a.cfg = *cfg; a.tree = *tree; a.root_state = root_state;
-    a.ctl = (mwave::Control*)(ws + l.ctl);
-    a.paths = (int32_t*)(ws + l.paths);
-    a.plen = (int32_t*)(ws + l.plen);
-    a.expands = (int32_t*)(ws + l.expands);
-    a.recip = (double*)(ws + l.recip);
     a.plan = plan; a.result = result;
-    B2_CUDA_CHECK(cudaMemsetAsync(a.ctl, 0, sizeof(mwave::Control), stream));
-    const size_t smem = (size_t)mwave::TABLE_KEYS * 8;
-    B2_CUDA_CHECK(cudaFuncSetAttribute(mwave::mcts_wave_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int per_sm = 0;
-    B2_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, mwave::mcts_wave_kernel, mwave::THREADS, smem));
-    B2_REQUIRE(per_sm >= 1, "wave kernel does not fit on an SM");
-    int grid = sm_count();
-    if (cfg->max_ctas > 0 && cfg->max_ctas < grid) grid = cfg->max_ctas;
-    void* params[] = {&a};
-    B2_CUDA_CHECK(cudaLaunchCooperativeKernel((const void*)mwave::mcts_wave_kernel, dim3(grid), dim3(mwave::THREADS), params,
-                                              smem, stream));
-    return B2_OK;
+    return launch_wave<false>(cfg, a, workspace, (cudaStream_t)stream_);
+}
+
+extern "C" int b2_mcts_plan_wave_sampled(const b2_mcts_wave_config* cfg, const b2_finite_mdp_sampled* mdp,
+                                         const uint8_t* terminal, int32_t env_draws, const uint64_t* env_rng,
+                                         const int32_t* root_state, const b2_mcts_wave_tree* tree, void* workspace,
+                                         int8_t* plan, int32_t* result, int32_t* rejected, void* stream_) {
+    B2_REQUIRE(cfg && mdp && env_rng && root_state && tree && workspace && plan && result && rejected, "null pointer");
+    B2_REQUIRE(cfg->env_kind == B2_ENV_FINITE, "env_kind must be B2_ENV_FINITE");
+    if (check_wave_config(cfg) != B2_OK) return B2_ERR_INVALID;
+    if (check_sampled_mdp(*mdp, cfg->n_actions, terminal, true) != B2_OK) return B2_ERR_INVALID;
+    B2_REQUIRE(env_draws == 0 || env_draws == 1, "env_draws must be 0 or 1");
+    mwave::Args a;
+    a.cfg = *cfg; a.tree = *tree; a.root_state = root_state;
+    a.plan = plan; a.result = result;
+    a.smdp = *mdp; a.terminal = terminal; a.env_draws = env_draws; a.env_rng = env_rng; a.rejected = rejected;
+    return launch_wave<true>(cfg, a, workspace, (cudaStream_t)stream_);
 }

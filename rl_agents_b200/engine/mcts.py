@@ -1,8 +1,13 @@
-"""Batched MCTS engine (device side of MCTSAgent)."""
+"""Batched MCTS engine (device side of MCTSAgent).
+
+A finite MDP in mode "deterministic" runs b2_mcts_plan / b2_mcts_plan_wave on FiniteTables; in mode "stochastic" or
+"sparse" it runs b2_mcts_plan_sampled / b2_mcts_plan_wave_sampled on SampledFiniteTables.  The reference never reseeds
+its env copies, so those take the live env's generator words (`env_words`), which every episode's copy starts from."""
 import numpy as np
 
 from rl_agents_b200 import _lib
-from rl_agents_b200.engine.tables import FiniteTables, gamma_tables, preference_tables, uniform_cdf_table
+from rl_agents_b200.engine.tables import (FiniteTables, SampledFiniteTables, gamma_tables, preference_tables,
+                                          uniform_cdf_table)
 from rl_agents_b200.engine.tree_engine import TreeEngine, decode_action
 
 POLICIES = {"random_available": 0, "random": 1, "preference": 2}
@@ -87,29 +92,54 @@ class MCTSEngine(TreeEngine):
         gp, _ = gamma_tables(gamma, self.horizon + 1)
         self.gamma_pow = torch.as_tensor(gp, device=self.device)
         self.cdf = torch.as_tensor(uniform_cdf_table(self.n_actions), device=self.device)
-        self.tables = FiniteTables(mdp, self.device) if env_kind == _lib.ENV_FINITE else None
+        self.sampled = env_kind == _lib.ENV_FINITE and mdp.mode != "deterministic"
+        self.tables = None
+        if self.sampled:
+            self.tables = SampledFiniteTables(mdp, self.device)
+            self.env_rng = torch.empty((self.n_trees, _lib.PCG64_STATE_WORDS), dtype=torch.int64, device=self.device)
+        elif env_kind == _lib.ENV_FINITE:
+            self.tables = FiniteTables(mdp, self.device)
         self.tree = _lib.MCTSTree(*self._alloc_tree(_lib.MCTS_TREE_FIELDS, self.capacity))
         self.pref_prior = torch.as_tensor(preference_tables(self.n_actions, prior_ratio)[0], device=self.device)
         self.pref_cdf = torch.as_tensor(preference_tables(self.n_actions, rollout_ratio)[1], device=self.device)
         self.cfg = _lib.MCTSConfig(env_kind, self.n_trees, self.n_actions, self.episodes, self.horizon, self.capacity,
                                    rollout_id, prior_id, float(temperature),
                                    self.gamma_pow.data_ptr(), self.cdf.data_ptr(),
-                                   self.tables.struct() if self.tables else _lib.FiniteMDP(),
+                                   self.tables.struct() if self.tables and not self.sampled else _lib.FiniteMDP(),
                                    prior_action, rollout_action, self.pref_prior.data_ptr(), self.pref_cdf.data_ptr(), None)
         self.resume = torch.zeros(self.n_trees, dtype=torch.int32, device=self.device)
         self.plan_buf = torch.empty((self.n_trees, max(self.horizon, 1)), dtype=torch.int8, device=self.device)
 
-    def plan(self, root_states, rng_words, resume_nodes=None):
+    def plan(self, root_states, rng_words, resume_nodes=None, env_words=None):
         """rng_words: uint64 [n_trees, 6] numpy (pcg64_words per tree).  resume_nodes: per-tree node counts of
-        re-rooted sub-trees already in the arrays (see reroot), or None for fresh trees."""
+        re-rooted sub-trees already in the arrays (see reroot), or None for fresh trees.  env_words (sampled MDPs
+        only): uint64 [6] or [n_trees, 6], pcg64_words of the live env's generator that each tree's env copies start
+        from."""
         self._load_rng(rng_words)
         if resume_nodes is None:
             self.cfg.resume_nodes = None
         else:
             self.resume.copy_(self.torch.as_tensor(np.asarray(resume_nodes, dtype=np.int32)))
             self.cfg.resume_nodes = self.resume.data_ptr()
+        if self.sampled:
+            if env_words is None:
+                raise ValueError("MCTS on a stochastic finite MDP needs the env generator's words (env_words)")
+            w = np.array(np.broadcast_to(np.asarray(env_words, dtype=np.uint64), (self.n_trees, _lib.PCG64_STATE_WORDS)))
+            self.env_rng.copy_(self.torch.from_numpy(w.view(np.int64)))
+            t = self.tables
+            _lib.check(self.lib.b2_mcts_plan_sampled(
+                self.cfg, t.struct(), _lib.ptr(t.terminal), t.env_draws, _lib.ptr(self.env_rng),
+                _lib.ptr(root_states), self.tree, _lib.ptr(self.rng), _lib.ptr(self.plan_buf), _lib.ptr(self.result),
+                _lib.current_stream()))
+            return
         _lib.check(self.lib.b2_mcts_plan(self.cfg, _lib.ptr(root_states), self.tree, _lib.ptr(self.rng),
                                          _lib.ptr(self.plan_buf), _lib.ptr(self.result), _lib.current_stream()))
+
+    def _check(self, res):
+        if self.sampled:
+            bad = np.nonzero(res[:, 3] == 1)[0]
+            if bad.size:
+                self.tables.raise_rejected_row(int(res[bad[0], 4]))
 
     def _plans(self, res):
         plans = self.plan_buf.cpu().numpy()
@@ -152,7 +182,14 @@ class MCTSWaveEngine(object):
         self.capacity = 1 + self.episodes * self.n_actions
         gp, _ = gamma_tables(gamma, self.horizon + 1)
         self.gamma_pow = torch.as_tensor(gp, device=self.device)
-        self.tables = FiniteTables(mdp, self.device) if env_kind == _lib.ENV_FINITE else None
+        self.sampled = env_kind == _lib.ENV_FINITE and mdp.mode != "deterministic"
+        self.tables = None
+        if self.sampled:
+            self.tables = SampledFiniteTables(mdp, self.device)
+            self.env_rng = torch.empty(_lib.PCG64_STATE_WORDS, dtype=torch.int64, device=self.device)
+            self.rejected = torch.empty(2, dtype=torch.int32, device=self.device)
+        elif env_kind == _lib.ENV_FINITE:
+            self.tables = FiniteTables(mdp, self.device)
         i32 = torch.int32
         self.parent = torch.empty(self.capacity, dtype=i32, device=self.device)
         self.first_child = torch.empty(self.capacity, dtype=i32, device=self.device)
@@ -162,7 +199,8 @@ class MCTSWaveEngine(object):
         self.value = torch.empty(self.capacity, dtype=torch.float64, device=self.device)
         self.cfg = _lib.MCTSWaveConfig(env_kind, self.n_actions, self.episodes, self.horizon, self.capacity, self.width,
                                        0, 0, float(temperature), 0, self.gamma_pow.data_ptr(),
-                                       self.tables.struct() if self.tables else _lib.FiniteMDP(), int(max_ctas), 0)
+                                       self.tables.struct() if self.tables and not self.sampled else _lib.FiniteMDP(),
+                                       int(max_ctas), 0)
         self.tree = _lib.MCTSWaveTree(*[t.data_ptr() for t in (self.parent, self.first_child, self.count, self.meta,
                                                                self.vsum, self.value)])
         ws = self.lib.b2_mcts_wave_workspace_bytes(self.cfg)
@@ -172,15 +210,31 @@ class MCTSWaveEngine(object):
         self.plan_buf = torch.empty(max(self.horizon, 1), dtype=torch.int8, device=self.device)
         self.result = torch.empty(_lib.MCTS_RESULT_WORDS, dtype=i32, device=self.device)
 
-    def plan(self, root_state, seed):
-        """root_state: int32 device tensor [1] (finite) or [136]; seed: the counter-based generator's seed."""
+    def plan(self, root_state, seed, env_words=None):
+        """root_state: int32 device tensor [1] (finite) or [136]; seed: the counter-based generator's seed;
+        env_words (sampled MDPs only): uint64 [6], pcg64_words of the live env's generator."""
         assert root_state.dtype == self.torch.int32 and root_state.is_cuda and root_state.is_contiguous()
         self.cfg.seed = int(seed) & ((1 << 64) - 1)
+        if self.sampled:
+            if env_words is None:
+                raise ValueError("MCTS on a stochastic finite MDP needs the env generator's words (env_words)")
+            w = np.ascontiguousarray(np.asarray(env_words, dtype=np.uint64).reshape(-1))
+            self.env_rng.copy_(self.torch.from_numpy(w.view(np.int64)))
+            t = self.tables
+            _lib.check(self.lib.b2_mcts_plan_wave_sampled(
+                self.cfg, t.struct(), _lib.ptr(t.terminal), t.env_draws, _lib.ptr(self.env_rng), _lib.ptr(root_state),
+                self.tree, _lib.ptr(self.workspace), _lib.ptr(self.plan_buf), _lib.ptr(self.result),
+                _lib.ptr(self.rejected), _lib.current_stream()))
+            return
         _lib.check(self.lib.b2_mcts_plan_wave(self.cfg, _lib.ptr(root_state), self.tree, _lib.ptr(self.workspace),
                                               _lib.ptr(self.plan_buf), _lib.ptr(self.result), _lib.current_stream()))
 
     def finish(self):
         res = self.result.cpu().numpy()
+        if self.sampled:
+            episode, row = self.rejected.cpu().numpy().tolist()
+            if episode >= 0:
+                self.tables.raise_rejected_row(row)
         return self.plan_buf.cpu().numpy()[:res[1]].astype(int).tolist(), res
 
     def tree_dict(self):

@@ -7,14 +7,18 @@ from rl_agents_b200 import _lib
 
 
 class EnvDescription(object):
-    __slots__ = ("kind", "n_actions", "mdp", "root")
+    __slots__ = ("kind", "n_actions", "mdp", "root", "env_words")
 
 
-def describe(env):
-    """-> EnvDescription(kind, action_space.n, finite MDP tables or None, root state int32 array)."""
+def describe(env, env_words=False):
+    """-> EnvDescription(kind, action_space.n, finite MDP tables or None, root state int32 array, env_words).
+    env_words: with env_words set (the planners that step deep copies of the env without reseeding them: MCTS), for a
+    finite MDP in mode "stochastic" or "sparse", the uint64 [6] words (pcg64_words) of the env's own generator, which
+    such a copy steps with -- ValueError when that generator is not a numpy Generator(PCG64); None otherwise."""
     u = getattr(env, "unwrapped", env)
     d = EnvDescription()
     d.n_actions = int(env.action_space.n)
+    d.env_words = None
     kind = getattr(u, "b2_env_kind", None)
     if kind == "intersection":
         d.kind, d.mdp = _lib.ENV_INTERSECTION, None
@@ -35,6 +39,13 @@ def describe(env):
         # rl_agents_b200.envs.FiniteMDPEnv or the `finite_mdp` package's FiniteMDPEnv
         d.kind, d.mdp = _lib.ENV_FINITE, mdp
         d.root = np.array([int(mdp.state)], dtype=np.int32)
+        if env_words and getattr(mdp, "mode", "deterministic") != "deterministic":
+            from rl_agents_b200.engine.mcts import pcg64_words
+            gen = getattr(u, "np_random", None)
+            if not isinstance(gen, np.random.Generator) or not isinstance(gen.bit_generator, np.random.PCG64):
+                raise ValueError("a stochastic finite-MDP env must step with a numpy Generator(PCG64) "
+                                 "(got %r)" % (type(getattr(gen, "bit_generator", gen)).__name__,))
+            d.env_words = pcg64_words(gen)
         return d
     raise TypeError("rl_agents_b200 planners need a HighwayLiteEnv, a highway_env highway-v0 env or a finite-MDP env "
                     "(got %r); see INTEGRATION.md for the env hand-off" % type(u).__name__)
