@@ -30,6 +30,7 @@ struct BrueArgs {
     uint64_t* rng;
     int8_t* plan;
     int32_t* result;
+    LaneModel model;
 };
 
 __device__ __forceinline__ void new_node(const b2_brue_tree& tr, int64_t nb, int id, int parent, int action, int kind) {
@@ -69,13 +70,7 @@ __device__ double estimate(const b2_brue_tree& tr, int64_t nb, int node, int lev
 
 template <class Env>
 __global__ void __launch_bounds__(128, 8) brue_kernel(BrueArgs a) {
-    constexpr int G = Env::GROUP;
-    const int gtid = blockIdx.x * 128 + threadIdx.x;
-    const int tree = gtid / G, li = gtid % G;
-    if (tree >= a.cfg.n_trees) return;              // whole lane groups: no live lane of a group leaves here
-    const bool writer = li == 0;
-    const int lane = threadIdx.x & 31;
-    const unsigned gmask = G == 1 ? (1u << lane) : (0xFFFFu << (lane & 16));
+    B2_LANE_MAP_LIVE(Env, a.cfg.n_trees);          // whole lane groups: no live lane of a group leaves
     const int H = a.cfg.horizon;
     const int64_t nb = (int64_t)tree * a.cfg.node_capacity;
     const b2_brue_tree& tr = a.tree;
@@ -99,7 +94,9 @@ __global__ void __launch_bounds__(128, 8) brue_kernel(BrueArgs a) {
         for (int h = 0; h < H; ++h) {                // rollout (:24-33)
             const int action = (int)rng.integers((uint32_t)a.cfg.n_actions);
             bool term, trunc;
-            const double r = env.step(a.cfg.mdp, action, li, gmask, term, trunc);
+            double r;
+            int bad_row;
+            env.step(a.model, action, li, gmask, true, term, trunc, r, bad_row);
             if (writer) {                            // update's forward pass (:39-44)
                 // DecisionNode.get_child: the chance child of this action, appended to the list on the first visit
                 int c = tr.first_child[nb + node], last = -1;
@@ -192,10 +189,11 @@ extern "C" int b2_brue_plan(const b2_brue_config* cfg, const int32_t* root_state
     cudaStream_t stream = (cudaStream_t)stream_;
     BrueArgs a;
     a.cfg = *cfg; a.tree = *tree; a.root_states = root_states; a.rng = rng; a.plan = plan; a.result = result;
+    a.model = LaneModel{cfg->mdp};
     if (cfg->env_kind == B2_ENV_FINITE)
-        brue_kernel<FiniteEnv><<<lane_grid(cfg->n_trees, FiniteEnv::GROUP), 128, 0, stream>>>(a);
+        brue_kernel<FiniteEnv><<<lane_grid<FiniteEnv>(cfg->n_trees), 128, 0, stream>>>(a);
     else
-        brue_kernel<HighwayEnv><<<lane_grid(cfg->n_trees, HighwayEnv::GROUP), 128, 0, stream>>>(a);
+        brue_kernel<HighwayEnv><<<lane_grid<HighwayEnv>(cfg->n_trees), 128, 0, stream>>>(a);
     B2_CUDA_CHECK(cudaGetLastError());
     return B2_OK;
 }

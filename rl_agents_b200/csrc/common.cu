@@ -50,6 +50,14 @@ int check_sampled_mdp(const b2_finite_mdp_sampled& mdp, int n_actions, const uin
     B2_REQUIRE(mdp.n_actions == n_actions && mdp.n_states > 0 && mdp.n_next >= 1, "bad finite MDP shape");
     return B2_OK;
 }
+
+int check_sampled_entry(int env_kind, const b2_finite_mdp_sampled& mdp, int n_actions, const uint8_t* terminal,
+                        int32_t env_draws) {
+    B2_REQUIRE(env_kind == B2_ENV_FINITE, "env_kind must be B2_ENV_FINITE");
+    if (check_sampled_mdp(mdp, n_actions, terminal, true) != B2_OK) return B2_ERR_INVALID;
+    B2_REQUIRE(env_draws == 0 || env_draws == 1, "env_draws must be 0 or 1");
+    return B2_OK;
+}
 }  // namespace b2
 
 extern "C" const char* b2_last_error(void) { return b2::g_err; }

@@ -41,9 +41,15 @@ int check_lane_env_il(int env_kind, int n_actions, const b2_finite_mdp& mdp);
 // B2_OK, or B2_ERR_INVALID with the error set.  Its tables, and terminal when the planner reads it (needs_terminal),
 // then its shape against the planner's n_actions.
 int check_sampled_mdp(const b2_finite_mdp_sampled& mdp, int n_actions, const uint8_t* terminal, bool needs_terminal);
+// The launch check the *_sampled entry points (MCTS per tree and wavefront, OLOP, MDP-GapE) share after their own
+// config checks: B2_OK, or B2_ERR_INVALID with the error set.  A finite env_kind, check_sampled_mdp with terminal,
+// and env_draws 0 or 1.
+int check_sampled_entry(int env_kind, const b2_finite_mdp_sampled& mdp, int n_actions, const uint8_t* terminal,
+                        int32_t env_draws);
 
-// Blocks of 128 threads for n_trees trees of `group` lanes each.
-inline int lane_grid(int n_trees, int group) { return (n_trees * group + 127) / 128; }
+// Blocks of 128 threads for n_trees trees of Env::GROUP lanes each.
+template <class Env>
+inline int lane_grid(int n_trees) { return (n_trees * Env::GROUP + 127) / 128; }
 
 // Grid-wide barrier of a cooperative launch (all CTAs co-resident), keyed on two control words of `ctl` that the launch
 // wrapper zeroes: the arrival count `bar_count` and the generation `bar_gen`.  Data written before it by any CTA is

@@ -1,14 +1,15 @@
 // Device env models of the one-tree-per-lane-group planners (mcts.cu, olop.cu, mdp_gape.cu, brue.cu, mcts_dpw.cu): one
 // tree per lane on a finite MDP, one tree per 16-lane group on HighwayLite and IntersectionLite (lane = vehicle slot, the
-// scene in registers, so the reference's deep copy of the env is a register copy).  Each model reads only what it
-// needs: the finite tables, the root states and the action count.
+// scene in registers, so the reference's deep copy of the env is a register copy).  B2_LANE_MAP places a thread in
+// its group; each model reads only what it needs: the launch's LaneModel, the root states and the action count.
 //
-// step() reports truncation separately; MCTS reads it, the other planners pass a dummy (the reference's 4-tuple step
-// drops truncation).
+// Every model has the same step(); it reports truncation separately; MCTS reads it, the other planners ignore it (the
+// reference's 4-tuple step drops truncation).  seed() and load_rng() set the env generator of SampledFiniteEnv and do
+// nothing on the deterministic models.
 //
 // A b2_finite_mdp_sampled row is sampled with sampled_next().  The planners that keep one env generator per episode
-// (olop.cu, mdp_gape.cu, mcts_dpw.cu) step SampledFiniteEnv with its step(); PlaTyPOOS (platypoos.cu) and sparse
-// sampling (sparse_sampling.cu) seed a fresh generator per child or sample and check row_ok in their own loops.
+// (mcts.cu, olop.cu, mdp_gape.cu, mcts_dpw.cu) step SampledFiniteEnv with its step(); PlaTyPOOS (platypoos.cu) and
+// sparse sampling (sparse_sampling.cu) seed a fresh generator per child or sample and check row_ok in their own loops.
 #pragma once
 #include <type_traits>
 
@@ -18,6 +19,43 @@
 #include "pcg64.cuh"
 
 namespace b2 {
+
+// The lane mapping of a lane-group kernel of 128-thread blocks, declared as the kernel's locals: tree = thread /
+// Env::GROUP and li = its lane in the group; writer: lane 0 of the group; gmask: the group's lanes in the warp (one
+// lane on a finite MDP, a half warp on HighwayLite and IntersectionLite).  B2_LANE_MAP keeps the threads of a group
+// past n_trees (live false): they shadow the last tree and never store.  B2_LANE_MAP_LIVE returns from them.
+// Macros, not a value type or helper function: inlining one, even with the same statements in the same order, changes
+// how ptxas assigns the registers of mcts_kernel<HighwayEnv>, and moving the early return after the shadowing form
+// changes the code of the four kernels that return.
+#define B2_LANE_GTID(Env)                                                         \
+    constexpr int G = Env::GROUP;                                                 \
+    const int gtid = blockIdx.x * 128 + threadIdx.x
+#define B2_LANE_GMASK                                                             \
+    const int lane = threadIdx.x & 31;                                            \
+    const unsigned gmask = G == 1 ? (1u << lane) : (0xFFFFu << (lane & 16))
+#define B2_LANE_MAP(Env, n_trees)                                                 \
+    B2_LANE_GTID(Env);                                                            \
+    const int tree_raw = gtid / G, li = gtid % G;                                 \
+    const bool live = tree_raw < (n_trees);                                       \
+    const int tree = live ? tree_raw : (n_trees) - 1;                             \
+    const bool writer = live && li == 0;                                          \
+    B2_LANE_GMASK
+#define B2_LANE_MAP_LIVE(Env, n_trees)                                            \
+    B2_LANE_GTID(Env);                                                            \
+    const int tree = gtid / G, li = gtid % G;                                     \
+    if (tree >= (n_trees)) return;                                                \
+    const bool writer = li == 0;                                                  \
+    B2_LANE_GMASK
+
+// The finite model of one launch, as every lane env's step() reads it: the deterministic tables (FiniteEnv), or the
+// sampled tables, terminal and whether a step draws from the env generator (SampledFiniteEnv).  HighwayLite and
+// IntersectionLite read none of it.
+struct LaneModel {
+    b2_finite_mdp mdp;
+    b2_finite_mdp_sampled smdp;
+    const uint8_t* terminal;
+    int32_t draws;
+};
 
 // searchsorted(cdf, u, side="right") on a non-decreasing row: the number of entries <= u
 __device__ __forceinline__ int searchsorted_right(const double* cdf, int n, double u) {
@@ -38,7 +76,13 @@ __device__ __forceinline__ int sampled_next(const b2_finite_mdp_sampled& m, int6
     return m.next[row * B + k];
 }
 
-struct FiniteEnv {
+// The env generator of a deterministic model: there is none to seed or load.
+struct NoEnvRng {
+    __device__ __forceinline__ void seed(const LaneModel& m, uint32_t seed) {}
+    __device__ __forceinline__ void load_rng(const uint64_t* words) {}
+};
+
+struct FiniteEnv : NoEnvRng {
     static constexpr int GROUP = 1;
     int s;
     __device__ __forceinline__ void load_root(const int32_t* root_states, int tree, int li) { s = root_states[tree]; }
@@ -46,30 +90,40 @@ struct FiniteEnv {
     __device__ __forceinline__ static int nth(int mask, int n) { return n; }
     // position of `action` among the available actions in the env's order, or -1
     __device__ __forceinline__ static int rank_of(int mask, int action) { return (action >= 0 && (mask >> action) & 1) ? action : -1; }
-    __device__ __forceinline__ double step(const b2_finite_mdp& m, int action, int li, unsigned gmask,
-                                           bool& term, bool& trunc) {
-        const double r = m.reward[(int64_t)s * m.n_actions + action];
-        term = m.terminal[s] != 0;        // finite_mdp's MDP.step: done = terminal[state BEFORE the transition]
-        s = m.transition[(int64_t)s * m.n_actions + action];
+    // Steps every lane, whatever `taken` says; never fails.
+    __device__ __forceinline__ bool step(const LaneModel& m, int action, int li, unsigned gmask, bool taken,
+                                         bool& term, bool& trunc, double& r, int& bad_row) {
+        r = m.mdp.reward[(int64_t)s * m.mdp.n_actions + action];
+        term = m.mdp.terminal[s] != 0;    // finite_mdp's MDP.step: done = terminal[state BEFORE the transition]
+        s = m.mdp.transition[(int64_t)s * m.mdp.n_actions + action];
         trunc = false;
-        return r;
+        return true;
     }
 };
 
-// A finite MDP in any mode, stepped as FiniteMDPEnv.step with the episode's env generator (env_rng; seeded by the
-// planner only when draw is set).  kSampled<Env> selects the code that calls this step().
+// A finite MDP in any mode, stepped as FiniteMDPEnv.step with the episode's env generator env_rng.  kSampled<Env>
+// selects what only the planners' sampled instantiations do.
 struct SampledFiniteEnv : FiniteEnv {
     Pcg64 env_rng;
-    // FiniteMDPEnv.step on row s * n_actions + action.  With draw set, a row Generator.choice rejects (its ValueError)
-    // returns false with bad_row = the row and s unchanged.  Otherwise term = terminal[state BEFORE the transition],
-    // r = reward[row], and sampled_next() moves s.
-    __device__ __forceinline__ bool step(const b2_finite_mdp_sampled& m, const uint8_t* terminal, bool draw, int action,
-                                         bool& term, double& r, int& bad_row) {
-        const int64_t row = (int64_t)s * m.n_actions + action;
-        if (draw && !m.row_ok[row]) { bad_row = (int)row; return false; }
-        term = terminal[s] != 0;
-        r = m.reward[row];
-        s = sampled_next(m, row, draw, env_rng);
+    // the env copy's state.seed(seed): default_rng(seed) when the steps draw
+    __device__ __forceinline__ void seed(const LaneModel& m, uint32_t seed) { if (m.draws) env_rng.seed_from(seed); }
+    __device__ __forceinline__ void load_rng(const uint64_t* words) { env_rng.load(words); }
+    // FiniteMDPEnv.step on row s * n_actions + action, for a step the reference takes; any other step leaves s and
+    // env_rng alone.  When the steps draw, a row Generator.choice rejects (its ValueError) returns false with
+    // bad_row = the row and s unchanged.  Otherwise term = terminal[state BEFORE the transition], r = reward[row], and
+    // sampled_next() moves s.
+    __device__ __forceinline__ bool step(const LaneModel& m, int action, int li, unsigned gmask, bool taken,
+                                         bool& term, bool& trunc, double& r, int& bad_row) {
+        const bool draw = m.draws != 0;
+        term = false;
+        trunc = false;
+        r = 0.0;
+        if (!taken) return true;
+        const int64_t row = (int64_t)s * m.smdp.n_actions + action;
+        if (draw && !m.smdp.row_ok[row]) { bad_row = (int)row; return false; }
+        term = m.terminal[s] != 0;
+        r = m.smdp.reward[row];
+        s = sampled_next(m.smdp, row, draw, env_rng);
         return true;
     }
 };
@@ -77,7 +131,7 @@ struct SampledFiniteEnv : FiniteEnv {
 template <class Env>
 constexpr bool kSampled = std::is_same<Env, SampledFiniteEnv>::value;
 
-struct HighwayEnv {
+struct HighwayEnv : NoEnvRng {
     static constexpr int GROUP = 16;
     hw::Lane L;
     int t, si;
@@ -100,15 +154,16 @@ struct HighwayEnv {
         }
         return -1;
     }
-    __device__ __forceinline__ double step(const b2_finite_mdp& m, int action, int li, unsigned gmask,
-                                           bool& term, bool& trunc) {
-        return (double)hw::step(L, li, t, si, action, term, trunc, gmask);
+    __device__ __forceinline__ bool step(const LaneModel& m, int action, int li, unsigned gmask, bool taken,
+                                         bool& term, bool& trunc, double& r, int& bad_row) {
+        r = (double)hw::step(L, li, t, si, action, term, trunc, gmask);
+        return true;
     }
 };
 
 // IntersectionLite (mcts.cu and olop.cu only): the same 16-lane group and 136-word slot as HighwayLite; three actions
 // offered in the env's order IDLE, FASTER, SLOWER, which is not ascending action id.
-struct IntersectionEnv {
+struct IntersectionEnv : NoEnvRng {
     static constexpr int GROUP = 16;
     il::Lane L;
     il::Globals g;
@@ -128,9 +183,10 @@ struct IntersectionEnv {
         }
         return -1;
     }
-    __device__ __forceinline__ double step(const b2_finite_mdp& m, int action, int li, unsigned gmask,
-                                           bool& term, bool& trunc) {
-        return (double)il::step(L, li, g, action, term, trunc, gmask);
+    __device__ __forceinline__ bool step(const LaneModel& m, int action, int li, unsigned gmask, bool taken,
+                                         bool& term, bool& trunc, double& r, int& bad_row) {
+        r = (double)il::step(L, li, g, action, term, trunc, gmask);
+        return true;
     }
 };
 

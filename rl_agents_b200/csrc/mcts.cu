@@ -30,11 +30,8 @@ struct MctsArgs {
     uint64_t* rng;
     int8_t* plan;
     int32_t* result;
-    // SampledFiniteEnv only
-    b2_finite_mdp_sampled smdp;
-    const uint8_t* terminal;
-    int32_t env_draws;
-    const uint64_t* env_rng;
+    const uint64_t* env_rng;   // SampledFiniteEnv: the env generator's words of each tree
+    LaneModel model;
 };
 
 // --------------------------------------------------------------- kernel ---
@@ -43,14 +40,7 @@ struct MctsArgs {
 #endif
 template <class Env>
 __global__ void __launch_bounds__(128, B2_MCTS_MIN_BLOCKS) mcts_kernel(MctsArgs a) {
-    constexpr int G = Env::GROUP;
-    const int gtid = blockIdx.x * 128 + threadIdx.x;
-    const int tree_raw = gtid / G, li = gtid % G;
-    const bool live = tree_raw < a.cfg.n_trees;
-    const int tree = live ? tree_raw : a.cfg.n_trees - 1;   // idle groups shadow the last tree, never store
-    const bool writer = live && li == 0;
-    const int lane = threadIdx.x & 31;
-    const unsigned gmask = G == 1 ? (1u << lane) : (0xFFFFu << (lane & 16));
+    B2_LANE_MAP(Env, a.cfg.n_trees);
     const int A = a.cfg.n_actions, H = a.cfg.horizon;
     const int64_t nb = (int64_t)tree * a.cfg.node_capacity;
     const b2_mcts_tree& tr = a.tree;
@@ -67,10 +57,10 @@ __global__ void __launch_bounds__(128, B2_MCTS_MIN_BLOCKS) mcts_kernel(MctsArgs 
     int error = 0, bad_row = -1;
 
     for (int ep = 0; ep < a.cfg.episodes; ++ep) {
-        if constexpr (kSampled<Env>) { if (error) break; }
+        if (error) break;
         Env env;
         env.load_root(a.root_states, tree, li);     // safe_deepcopy_env(state), mcts.py:183
-        if constexpr (kSampled<Env>) env.env_rng.load(a.env_rng + (int64_t)tree * B2_PCG64_STATE_WORDS);
+        env.load_rng(a.env_rng + (int64_t)tree * B2_PCG64_STATE_WORDS);
         int node = 0;
         bool in_sel = true, active = live;
         double total = 0.0;
@@ -151,15 +141,9 @@ __global__ void __launch_bounds__(128, B2_MCTS_MIN_BLOCKS) mcts_kernel(MctsArgs 
             bool term, trunc;
             Env next = env;
             double r;
-            if constexpr (kSampled<Env>) {
-                // only a step the reference takes draws or checks its row
-                r = 0.0; term = false; trunc = false;
-                if (active && !next.step(a.smdp, a.terminal, a.env_draws != 0, action, term, r, bad_row)) {
-                    error = ERR_BAD_ROW;
-                    active = false;
-                }
-            } else {
-                r = next.step(a.cfg.mdp, action, li, gmask, term, trunc);
+            if (!next.step(a.model, action, li, gmask, active, term, trunc, r, bad_row)) {
+                error = ERR_BAD_ROW;
+                active = false;
             }
             if (active) {
                 env = next;
@@ -237,12 +221,13 @@ extern "C" int b2_mcts_plan(const b2_mcts_config* cfg, const int32_t* root_state
     cudaStream_t stream = (cudaStream_t)stream_;
     MctsArgs a;
     a.cfg = *cfg; a.tree = *tree; a.root_states = root_states; a.rng = rng; a.plan = plan; a.result = result;
+    a.model = LaneModel{cfg->mdp};
     if (cfg->env_kind == B2_ENV_FINITE)
-        mcts_kernel<FiniteEnv><<<lane_grid(cfg->n_trees, FiniteEnv::GROUP), 128, 0, stream>>>(a);
+        mcts_kernel<FiniteEnv><<<lane_grid<FiniteEnv>(cfg->n_trees), 128, 0, stream>>>(a);
     else if (cfg->env_kind == B2_ENV_HIGHWAY)
-        mcts_kernel<HighwayEnv><<<lane_grid(cfg->n_trees, HighwayEnv::GROUP), 128, 0, stream>>>(a);
+        mcts_kernel<HighwayEnv><<<lane_grid<HighwayEnv>(cfg->n_trees), 128, 0, stream>>>(a);
     else
-        mcts_kernel<IntersectionEnv><<<lane_grid(cfg->n_trees, IntersectionEnv::GROUP), 128, 0, stream>>>(a);
+        mcts_kernel<IntersectionEnv><<<lane_grid<IntersectionEnv>(cfg->n_trees), 128, 0, stream>>>(a);
     B2_CUDA_CHECK(cudaGetLastError());
     return B2_OK;
 }
@@ -252,15 +237,13 @@ extern "C" int b2_mcts_plan_sampled(const b2_mcts_config* cfg, const b2_finite_m
                                     const b2_mcts_tree* tree, uint64_t* rng, int8_t* plan, int32_t* result,
                                     void* stream_) {
     B2_REQUIRE(cfg && mdp && env_rng && root_states && tree && rng && plan && result, "null pointer");
-    B2_REQUIRE(cfg->env_kind == B2_ENV_FINITE, "env_kind must be B2_ENV_FINITE");
     if (check_mcts_config(cfg) != B2_OK) return B2_ERR_INVALID;
-    if (check_sampled_mdp(*mdp, cfg->n_actions, terminal, true) != B2_OK) return B2_ERR_INVALID;
-    B2_REQUIRE(env_draws == 0 || env_draws == 1, "env_draws must be 0 or 1");
+    if (check_sampled_entry(cfg->env_kind, *mdp, cfg->n_actions, terminal, env_draws) != B2_OK) return B2_ERR_INVALID;
     cudaStream_t stream = (cudaStream_t)stream_;
     MctsArgs a;
     a.cfg = *cfg; a.tree = *tree; a.root_states = root_states; a.rng = rng; a.plan = plan; a.result = result;
-    a.smdp = *mdp; a.terminal = terminal; a.env_draws = env_draws; a.env_rng = env_rng;
-    mcts_kernel<SampledFiniteEnv><<<lane_grid(cfg->n_trees, SampledFiniteEnv::GROUP), 128, 0, stream>>>(a);
+    a.env_rng = env_rng; a.model = LaneModel{b2_finite_mdp{}, *mdp, terminal, env_draws};
+    mcts_kernel<SampledFiniteEnv><<<lane_grid<SampledFiniteEnv>(cfg->n_trees), 128, 0, stream>>>(a);
     B2_CUDA_CHECK(cudaGetLastError());
     return B2_OK;
 }

@@ -46,22 +46,8 @@ struct DpwArgs {
     uint64_t* rng;
     int8_t* plan;
     int32_t* result;
+    LaneModel model;
 };
-
-// Env::step on either model (the finite MDP with the run's env generator, HighwayLite deterministic); bad_row >= 0: the
-// finite row Generator.choice rejects
-template <class Env>
-__device__ __forceinline__ double dpw_step(Env& env, const b2_mcts_dpw_config& c, int action, int li, unsigned gmask,
-                                           bool& term, bool& trunc, int& bad_row) {
-    if constexpr (kSampled<Env>) {
-        double r = 0.0;
-        trunc = false;
-        env.step(c.mdp, c.terminal, c.env_draws != 0, action, term, r, bad_row);
-        return r;
-    } else {
-        return env.step(b2_finite_mdp{}, action, li, gmask, term, trunc);
-    }
-}
 
 // The observation's key: the state's on the finite MDP; on HighwayLite the step count t, which the host turns into
 // sha1(str(t))[:5] for the dump (the model is deterministic, so a chance node has one child either way).
@@ -83,13 +69,7 @@ __device__ __forceinline__ void new_node(const b2_mcts_dpw_tree& tr, int64_t nb,
 
 template <class Env>
 __global__ void __launch_bounds__(128, Env::GROUP == 16 ? 4 : 8) mcts_dpw_kernel(DpwArgs a) {
-    constexpr int G = Env::GROUP;
-    const int gtid = blockIdx.x * 128 + threadIdx.x;
-    const int tree = gtid / G, li = gtid % G;
-    if (tree >= a.cfg.n_trees) return;              // whole lane groups: no live lane of a group leaves here
-    const bool writer = li == 0;
-    const int lane = threadIdx.x & 31;
-    const unsigned gmask = G == 1 ? (1u << lane) : (0xFFFFu << (lane & 16));
+    B2_LANE_MAP_LIVE(Env, a.cfg.n_trees);          // whole lane groups: no live lane of a group leaves
     const b2_mcts_dpw_config& c = a.cfg;
     const b2_mcts_dpw_tree& tr = a.tree;
     const int A = c.n_actions, H = c.horizon;
@@ -105,8 +85,7 @@ __global__ void __launch_bounds__(128, Env::GROUP == 16 ? 4 : 8) mcts_dpw_kernel
         if (n_nodes + 2 > c.node_capacity) { error = ERR_CAPACITY; break; }
         Env env;
         env.load_root(a.root_states, tree, li);                       // safe_deepcopy_env(state), mcts.py:183
-        const uint32_t seed = rng.integers(1u << 30);                  // state.seed(np_random.randint(2**30)), :69
-        if constexpr (kSampled<Env>) { if (c.env_draws) env.env_rng.seed_from(seed); }
+        env.seed(a.model, rng.integers(1u << 30));                     // state.seed(np_random.randint(2**30)), :69
         int node = 0, depth = 0;
         bool term = false, trunc = false;
         double total = 0.0;
@@ -148,7 +127,8 @@ __global__ void __launch_bounds__(128, Env::GROUP == 16 ? 4 : 8) mcts_dpw_kernel
                 }
                 action = tr.key[nb + chance];
             }
-            const double r = dpw_step(env, c, action, li, gmask, term, trunc, bad_row);
+            double r;
+            env.step(a.model, action, li, gmask, true, term, trunc, r, bad_row);
             if (bad_row >= 0) { error = ERR_BAD_ROW; break; }
             ++steps;
             // ChanceNode.get_child (:171-182)
@@ -190,8 +170,9 @@ __global__ void __launch_bounds__(128, Env::GROUP == 16 ? 4 : 8) mcts_dpw_kernel
                 for (int i = 0; i < n; ++i) idx += cdf[i] <= u ? 1 : 0;   // searchsorted(side='right')
                 idx = min(idx, n - 1);
                 const int action = c.rollout_policy != 1 ? Env::nth(pm, idx) : idx;
-                const double r = dpw_step(env, c, action, li, gmask, term, trunc, bad_row);
-                if (bad_row >= 0) { error = ERR_BAD_ROW; break; }
+                double r;
+                env.step(a.model, action, li, gmask, true, term, trunc, r, bad_row);
+            if (bad_row >= 0) { error = ERR_BAD_ROW; break; }
                 ++steps;
                 total = total + c.gamma_pow[h] * r;
                 if (term || trunc) break;
@@ -262,12 +243,13 @@ extern "C" int b2_mcts_dpw_plan(const b2_mcts_dpw_config* cfg, const int32_t* ro
     cudaStream_t stream = (cudaStream_t)stream_;
     DpwArgs a;
     a.cfg = *cfg; a.tree = *tree; a.root_states = root_states; a.rng = rng; a.plan = plan; a.result = result;
+    a.model = LaneModel{b2_finite_mdp{}, cfg->mdp, cfg->terminal, cfg->env_draws};
     if (cfg->env_kind == B2_ENV_FINITE) {
         if (check_sampled_mdp(cfg->mdp, cfg->n_actions, cfg->terminal, true) != B2_OK) return B2_ERR_INVALID;
         B2_REQUIRE(!cfg->closed_loop || cfg->obs_keys, "observation key table missing");
-        mcts_dpw_kernel<SampledFiniteEnv><<<lane_grid(cfg->n_trees, SampledFiniteEnv::GROUP), 128, 0, stream>>>(a);
+        mcts_dpw_kernel<SampledFiniteEnv><<<lane_grid<SampledFiniteEnv>(cfg->n_trees), 128, 0, stream>>>(a);
     } else {
-        mcts_dpw_kernel<HighwayEnv><<<lane_grid(cfg->n_trees, HighwayEnv::GROUP), 128, 0, stream>>>(a);
+        mcts_dpw_kernel<HighwayEnv><<<lane_grid<HighwayEnv>(cfg->n_trees), 128, 0, stream>>>(a);
     }
     B2_CUDA_CHECK(cudaGetLastError());
     return B2_OK;

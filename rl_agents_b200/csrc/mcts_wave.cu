@@ -597,10 +597,8 @@ extern "C" int b2_mcts_plan_wave_sampled(const b2_mcts_wave_config* cfg, const b
                                          const int32_t* root_state, const b2_mcts_wave_tree* tree, void* workspace,
                                          int8_t* plan, int32_t* result, int32_t* rejected, void* stream_) {
     B2_REQUIRE(cfg && mdp && env_rng && root_state && tree && workspace && plan && result && rejected, "null pointer");
-    B2_REQUIRE(cfg->env_kind == B2_ENV_FINITE, "env_kind must be B2_ENV_FINITE");
     if (check_wave_config(cfg) != B2_OK) return B2_ERR_INVALID;
-    if (check_sampled_mdp(*mdp, cfg->n_actions, terminal, true) != B2_OK) return B2_ERR_INVALID;
-    B2_REQUIRE(env_draws == 0 || env_draws == 1, "env_draws must be 0 or 1");
+    if (check_sampled_entry(cfg->env_kind, *mdp, cfg->n_actions, terminal, env_draws) != B2_OK) return B2_ERR_INVALID;
     mwave::Args a;
     a.cfg = *cfg; a.tree = *tree; a.root_state = root_state;
     a.plan = plan; a.result = result;

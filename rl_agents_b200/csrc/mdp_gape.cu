@@ -43,11 +43,8 @@ struct GapeArgs {
     uint64_t* rng;
     int8_t* plan;
     int32_t* result;
-    // SampledFiniteEnv only
-    b2_finite_mdp_sampled smdp;
-    const uint8_t* terminal;
-    int32_t* keys;
-    int32_t env_draws;
+    int32_t* keys;             // SampledFiniteEnv: the state id each decision node was observed under
+    LaneModel model;
 };
 
 // ChanceNode.backup_to_root (mdp_gape.py:288-305) for one side: with f = u_next (upper) or -l_next (lower),
@@ -232,13 +229,7 @@ __device__ __forceinline__ void new_node(const b2_mdp_gape_tree& tr, int64_t nb,
 
 template <class Env>
 __global__ void __launch_bounds__(128, 8) mdp_gape_kernel(GapeArgs a) {
-    constexpr int G = Env::GROUP;
-    const int gtid = blockIdx.x * 128 + threadIdx.x;
-    const int tree = gtid / G, li = gtid % G;
-    if (tree >= a.cfg.n_trees) return;              // whole lane groups: no live lane of a group leaves here
-    const bool writer = li == 0;
-    const int lane = threadIdx.x & 31;
-    const unsigned gmask = G == 1 ? (1u << lane) : (0xFFFFu << (lane & 16));
+    B2_LANE_MAP_LIVE(Env, a.cfg.n_trees);          // whole lane groups: no live lane of a group leaves
     const int H = a.cfg.horizon, K = a.cfg.max_next_states;
     const int64_t nb = (int64_t)tree * a.cfg.node_capacity;
     const b2_mdp_gape_tree& tr = a.tree;
@@ -269,8 +260,7 @@ __global__ void __launch_bounds__(128, 8) mdp_gape_kernel(GapeArgs a) {
     while (!done) {                                  // MDPGapE.plan (:94-110)
         Env env;
         env.load_root(a.root_states, tree, li);      // safe_deepcopy_env(state), :98
-        const uint32_t seed = rng.integers(1u << 30);    // state.seed(np_random.randint(2**30)), :67
-        if constexpr (kSampled<Env>) { if (a.env_draws) env.env_rng.seed_from(seed); }
+        env.seed(a.model, rng.integers(1u << 30));       // state.seed(np_random.randint(2**30)), :67
         if (tr.first_child[nb] < 0) expand_decision(0, env.avail(a.cfg.n_actions, gmask), 0);
         int node = 0;
         for (int h = 0; h < H; ++h) {
@@ -312,13 +302,9 @@ __global__ void __launch_bounds__(128, 8) mdp_gape_kernel(GapeArgs a) {
             action = tr.meta[nb + chance] & 0xff;
             bool term, trunc;
             double r;                                                                        // :82
-            if constexpr (kSampled<Env>) {
-                if (!env.step(a.smdp, a.terminal, a.env_draws != 0, action, term, r, bad_row)) {
-                    error = ERR_BAD_ROW;
-                    break;
-                }
-            } else {
-                r = env.step(a.cfg.mdp, action, li, gmask, term, trunc);
+            if (!env.step(a.model, action, li, gmask, true, term, trunc, r, bad_row)) {
+                error = ERR_BAD_ROW;
+                break;
             }
             // ChanceNode.get_child (:272-286): placeholders on the first visit; a deterministic env observes placeholder 0
             int child = tr.first_child[nb + chance];
@@ -427,9 +413,7 @@ __global__ void __launch_bounds__(128, 8) mdp_gape_kernel(GapeArgs a) {
 
 using namespace b2;
 
-extern "C" int b2_mdp_gape_plan(const b2_mdp_gape_config* cfg, const int32_t* root_states, const b2_mdp_gape_tree* tree,
-                                uint64_t* rng, int8_t* plan, int32_t* result, void* stream_) {
-    B2_REQUIRE(cfg && root_states && tree && rng && plan && result, "null pointer");
+static int check_mdp_gape_config(const b2_mdp_gape_config* cfg) {
     B2_REQUIRE(cfg->n_trees > 0 && cfg->episodes >= 0 && cfg->horizon >= 1, "bad batch / budget");
     B2_REQUIRE(cfg->n_actions > 0 && cfg->n_actions <= 8, "n_actions must be in 1..8");
     B2_REQUIRE(cfg->max_next_states >= 1 && cfg->max_next_states <= 255, "max_next_states must be in 1..255");
@@ -438,15 +422,23 @@ extern "C" int b2_mdp_gape_plan(const b2_mdp_gape_config* cfg, const int32_t* ro
                "node_capacity too small");
     B2_REQUIRE(cfg->thresholds && cfg->transition_thresholds && cfg->init_upper,
                "threshold / initial bound tables missing");
+    return B2_OK;
+}
+
+extern "C" int b2_mdp_gape_plan(const b2_mdp_gape_config* cfg, const int32_t* root_states, const b2_mdp_gape_tree* tree,
+                                uint64_t* rng, int8_t* plan, int32_t* result, void* stream_) {
+    B2_REQUIRE(cfg && root_states && tree && rng && plan && result, "null pointer");
+    if (check_mdp_gape_config(cfg) != B2_OK) return B2_ERR_INVALID;
     const int rc = check_lane_env(cfg->env_kind, cfg->n_actions, cfg->mdp);
     if (rc != B2_OK) return rc;
     cudaStream_t stream = (cudaStream_t)stream_;
     GapeArgs a;
     a.cfg = *cfg; a.tree = *tree; a.root_states = root_states; a.rng = rng; a.plan = plan; a.result = result;
+    a.model = LaneModel{cfg->mdp};
     if (cfg->env_kind == B2_ENV_FINITE)
-        mdp_gape_kernel<FiniteEnv><<<lane_grid(cfg->n_trees, FiniteEnv::GROUP), 128, 0, stream>>>(a);
+        mdp_gape_kernel<FiniteEnv><<<lane_grid<FiniteEnv>(cfg->n_trees), 128, 0, stream>>>(a);
     else
-        mdp_gape_kernel<HighwayEnv><<<lane_grid(cfg->n_trees, HighwayEnv::GROUP), 128, 0, stream>>>(a);
+        mdp_gape_kernel<HighwayEnv><<<lane_grid<HighwayEnv>(cfg->n_trees), 128, 0, stream>>>(a);
     B2_CUDA_CHECK(cudaGetLastError());
     return B2_OK;
 }
@@ -456,22 +448,13 @@ extern "C" int b2_mdp_gape_plan_sampled(const b2_mdp_gape_config* cfg, const b2_
                                         const b2_mdp_gape_tree* tree, int32_t* keys, uint64_t* rng, int8_t* plan,
                                         int32_t* result, void* stream_) {
     B2_REQUIRE(cfg && mdp && terminal && root_states && tree && keys && rng && plan && result, "null pointer");
-    B2_REQUIRE(cfg->env_kind == B2_ENV_FINITE, "env_kind must be B2_ENV_FINITE");
-    B2_REQUIRE(cfg->n_trees > 0 && cfg->episodes >= 0 && cfg->horizon >= 1, "bad batch / budget");
-    B2_REQUIRE(cfg->n_actions > 0 && cfg->n_actions <= 8, "n_actions must be in 1..8");
-    if (check_sampled_mdp(*mdp, cfg->n_actions, terminal, true) != B2_OK) return B2_ERR_INVALID;
-    B2_REQUIRE(env_draws == 0 || env_draws == 1, "env_draws must be 0 or 1");
-    B2_REQUIRE(cfg->max_next_states >= 1 && cfg->max_next_states <= 255, "max_next_states must be in 1..255");
-    B2_REQUIRE((int64_t)cfg->node_capacity >= 1 + ((int64_t)cfg->episodes + 2) * cfg->horizon *
-                                                      (cfg->n_actions + cfg->max_next_states),
-               "node_capacity too small");
-    B2_REQUIRE(cfg->thresholds && cfg->transition_thresholds && cfg->init_upper,
-               "threshold / initial bound tables missing");
+    if (check_mdp_gape_config(cfg) != B2_OK) return B2_ERR_INVALID;
+    if (check_sampled_entry(cfg->env_kind, *mdp, cfg->n_actions, terminal, env_draws) != B2_OK) return B2_ERR_INVALID;
     cudaStream_t stream = (cudaStream_t)stream_;
     GapeArgs a;
     a.cfg = *cfg; a.tree = *tree; a.root_states = root_states; a.rng = rng; a.plan = plan; a.result = result;
-    a.smdp = *mdp; a.terminal = terminal; a.keys = keys; a.env_draws = env_draws;
-    mdp_gape_kernel<SampledFiniteEnv><<<lane_grid(cfg->n_trees, 1), 128, 0, stream>>>(a);
+    a.keys = keys; a.model = LaneModel{b2_finite_mdp{}, *mdp, terminal, env_draws};
+    mdp_gape_kernel<SampledFiniteEnv><<<lane_grid<SampledFiniteEnv>(cfg->n_trees), 128, 0, stream>>>(a);
     B2_CUDA_CHECK(cudaGetLastError());
     return B2_OK;
 }

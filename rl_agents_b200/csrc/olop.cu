@@ -31,22 +31,12 @@ struct OlopArgs {
     uint64_t* rng;
     int8_t* plan;
     int32_t* result;
-    // SampledFiniteEnv only
-    b2_finite_mdp_sampled smdp;
-    const uint8_t* terminal;
-    int32_t env_draws;
+    LaneModel model;
 };
 
 template <class Env>
 __global__ void __launch_bounds__(128, 8) olop_kernel(OlopArgs a) {
-    constexpr int G = Env::GROUP;
-    const int gtid = blockIdx.x * 128 + threadIdx.x;
-    const int tree_raw = gtid / G, li = gtid % G;
-    const bool live = tree_raw < a.cfg.n_trees;
-    const int tree = live ? tree_raw : a.cfg.n_trees - 1;
-    const bool writer = live && li == 0;
-    const int lane = threadIdx.x & 31;
-    const unsigned gmask = G == 1 ? (1u << lane) : (0xFFFFu << (lane & 16));
+    B2_LANE_MAP(Env, a.cfg.n_trees);
     const int L = a.cfg.horizon;
     const int64_t nb = (int64_t)tree * a.cfg.node_capacity;
     const b2_olop_tree& tr = a.tree;
@@ -64,10 +54,7 @@ __global__ void __launch_bounds__(128, 8) olop_kernel(OlopArgs a) {
     for (int ep = 0; ep < a.cfg.episodes; ++ep) {
         Env env;
         env.load_root(a.root_states, tree, li);     // safe_deepcopy_env(state), olop.py:98
-        if (live) {
-            const uint32_t seed = rng.integers(1u << 30);    // state.seed(np_random.randint(2**30)), :73
-            if constexpr (kSampled<Env>) { if (a.env_draws) env.env_rng.seed_from(seed); }
-        }
+        if (live) env.seed(a.model, rng.integers(1u << 30));    // state.seed(np_random.randint(2**30)), :73
         int node = 0;
         const double threshold = a.cfg.thresholds[ep];
         for (int h = 0; h < L; ++h) {
@@ -114,14 +101,7 @@ __global__ void __launch_bounds__(128, 8) olop_kernel(OlopArgs a) {
             }
             bool term, trunc;
             double r;                                                                   // olop.py:87
-            if constexpr (kSampled<Env>) {
-                r = 0.0;
-                term = false;
-                if (live && !error && !env.step(a.smdp, a.terminal, a.env_draws != 0, action, term, r, bad_row))
-                    error = ERR_BAD_ROW;
-            } else {
-                r = env.step(a.cfg.mdp, action, li, gmask, term, trunc);
-            }
+            if (!env.step(a.model, action, li, gmask, live && !error, term, trunc, r, bad_row)) error = ERR_BAD_ROW;
             if (live && !error) {
                 node = child;
                 // update (olop.py:132-142)
@@ -191,25 +171,31 @@ __global__ void __launch_bounds__(128, 8) olop_kernel(OlopArgs a) {
 
 using namespace b2;
 
-extern "C" int b2_olop_plan(const b2_olop_config* cfg, const int32_t* root_states, const b2_olop_tree* tree,
-                            uint64_t* rng, int8_t* plan, int32_t* result, void* stream_) {
-    B2_REQUIRE(cfg && root_states && tree && rng && plan && result, "null pointer");
+static int check_olop_config(const b2_olop_config* cfg) {
     B2_REQUIRE(cfg->n_trees > 0 && cfg->episodes >= 0 && cfg->horizon >= 1, "bad batch / budget");
     B2_REQUIRE(cfg->n_actions > 0 && cfg->n_actions <= 8, "n_actions must be in 1..8");
     B2_REQUIRE((int64_t)cfg->node_capacity >= 1 + (int64_t)cfg->episodes * cfg->horizon * cfg->n_actions,
                "node_capacity too small");
     B2_REQUIRE(cfg->thresholds && cfg->init_upper, "threshold / initial bound tables missing");
+    return B2_OK;
+}
+
+extern "C" int b2_olop_plan(const b2_olop_config* cfg, const int32_t* root_states, const b2_olop_tree* tree,
+                            uint64_t* rng, int8_t* plan, int32_t* result, void* stream_) {
+    B2_REQUIRE(cfg && root_states && tree && rng && plan && result, "null pointer");
+    if (check_olop_config(cfg) != B2_OK) return B2_ERR_INVALID;
     const int rc = check_lane_env_il(cfg->env_kind, cfg->n_actions, cfg->mdp);
     if (rc != B2_OK) return rc;
     cudaStream_t stream = (cudaStream_t)stream_;
     OlopArgs a;
     a.cfg = *cfg; a.tree = *tree; a.root_states = root_states; a.rng = rng; a.plan = plan; a.result = result;
+    a.model = LaneModel{cfg->mdp};
     if (cfg->env_kind == B2_ENV_FINITE)
-        olop_kernel<FiniteEnv><<<lane_grid(cfg->n_trees, FiniteEnv::GROUP), 128, 0, stream>>>(a);
+        olop_kernel<FiniteEnv><<<lane_grid<FiniteEnv>(cfg->n_trees), 128, 0, stream>>>(a);
     else if (cfg->env_kind == B2_ENV_HIGHWAY)
-        olop_kernel<HighwayEnv><<<lane_grid(cfg->n_trees, HighwayEnv::GROUP), 128, 0, stream>>>(a);
+        olop_kernel<HighwayEnv><<<lane_grid<HighwayEnv>(cfg->n_trees), 128, 0, stream>>>(a);
     else
-        olop_kernel<IntersectionEnv><<<lane_grid(cfg->n_trees, IntersectionEnv::GROUP), 128, 0, stream>>>(a);
+        olop_kernel<IntersectionEnv><<<lane_grid<IntersectionEnv>(cfg->n_trees), 128, 0, stream>>>(a);
     B2_CUDA_CHECK(cudaGetLastError());
     return B2_OK;
 }
@@ -219,19 +205,13 @@ extern "C" int b2_olop_plan_sampled(const b2_olop_config* cfg, const b2_finite_m
                                     const b2_olop_tree* tree, uint64_t* rng, int8_t* plan, int32_t* result,
                                     void* stream_) {
     B2_REQUIRE(cfg && mdp && terminal && root_states && tree && rng && plan && result, "null pointer");
-    B2_REQUIRE(cfg->env_kind == B2_ENV_FINITE, "env_kind must be B2_ENV_FINITE");
-    B2_REQUIRE(cfg->n_trees > 0 && cfg->episodes >= 0 && cfg->horizon >= 1, "bad batch / budget");
-    B2_REQUIRE(cfg->n_actions > 0 && cfg->n_actions <= 8, "n_actions must be in 1..8");
-    if (check_sampled_mdp(*mdp, cfg->n_actions, terminal, true) != B2_OK) return B2_ERR_INVALID;
-    B2_REQUIRE(env_draws == 0 || env_draws == 1, "env_draws must be 0 or 1");
-    B2_REQUIRE((int64_t)cfg->node_capacity >= 1 + (int64_t)cfg->episodes * cfg->horizon * cfg->n_actions,
-               "node_capacity too small");
-    B2_REQUIRE(cfg->thresholds && cfg->init_upper, "threshold / initial bound tables missing");
+    if (check_olop_config(cfg) != B2_OK) return B2_ERR_INVALID;
+    if (check_sampled_entry(cfg->env_kind, *mdp, cfg->n_actions, terminal, env_draws) != B2_OK) return B2_ERR_INVALID;
     cudaStream_t stream = (cudaStream_t)stream_;
     OlopArgs a;
     a.cfg = *cfg; a.tree = *tree; a.root_states = root_states; a.rng = rng; a.plan = plan; a.result = result;
-    a.smdp = *mdp; a.terminal = terminal; a.env_draws = env_draws;
-    olop_kernel<SampledFiniteEnv><<<lane_grid(cfg->n_trees, SampledFiniteEnv::GROUP), 128, 0, stream>>>(a);
+    a.model = LaneModel{b2_finite_mdp{}, *mdp, terminal, env_draws};
+    olop_kernel<SampledFiniteEnv><<<lane_grid<SampledFiniteEnv>(cfg->n_trees), 128, 0, stream>>>(a);
     B2_CUDA_CHECK(cudaGetLastError());
     return B2_OK;
 }

@@ -531,11 +531,13 @@ __global__ void __launch_bounds__(64) highway_step_groups_kernel(const int32_t* 
     for (int k = 0; k < n_steps[s]; ++k) {
         const int64_t o = (int64_t)s * max_steps + k;
         bool term, trunc;
-        const float r = (float)env.step(b2_finite_mdp{}, actions[o], li, gmask, term, trunc);
+        double r;
+        int bad_row;
+        env.step(LaneModel{}, actions[o], li, gmask, true, term, trunc, r, bad_row);
         const int avail = env.avail(hw::A_SLOWER + 1, gmask);
         hw::store_state(trace + o * hw::WORDS, li, env.L, env.t, env.si);
         if (li == 0) {
-            reward[o] = r;
+            reward[o] = (float)r;
             flags[o] = (term ? 1 : 0) | (trunc ? 2 : 0) | (avail << 2);
         }
     }

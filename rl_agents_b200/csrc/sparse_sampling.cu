@@ -178,13 +178,7 @@ struct SHighwayEnv {
 
 template <class Env>
 __global__ void __launch_bounds__(128, Env::GROUP == 16 ? 4 : 8) sparse_sampling_kernel(SsArgs a) {
-    constexpr int G = Env::GROUP;
-    const int gtid = blockIdx.x * 128 + threadIdx.x;
-    const int tree = gtid / G, li = gtid % G;
-    if (tree >= a.cfg.n_trees) return;              // whole lane groups: no live lane of a group leaves here
-    const bool writer = li == 0;
-    const int lane = threadIdx.x & 31;
-    const unsigned gmask = G == 1 ? (1u << lane) : (0xFFFFu << (lane & 16));
+    B2_LANE_MAP_LIVE(Env, a.cfg.n_trees);          // whole lane groups: no live lane of a group leaves
     const int H = a.cfg.horizon, C = a.cfg.C, n = a.cfg.n_trees, A = a.cfg.n_actions;
     const Stack& st = a.st;
     const b2_sparse_sampling_tree& tr = a.tree;
@@ -319,10 +313,10 @@ extern "C" int b2_sparse_sampling_plan(const b2_sparse_sampling_config* cfg, con
     if (cfg->env_kind == B2_ENV_FINITE) {
         if (check_sampled_mdp(cfg->mdp, cfg->n_actions, nullptr, false) != B2_OK) return B2_ERR_INVALID;
         layout((char*)workspace, cfg->n_trees, cfg->horizon, cfg->C, false, a.st);
-        sparse_sampling_kernel<SFiniteEnv><<<lane_grid(cfg->n_trees, SFiniteEnv::GROUP), 128, 0, stream>>>(a);
+        sparse_sampling_kernel<SFiniteEnv><<<lane_grid<SFiniteEnv>(cfg->n_trees), 128, 0, stream>>>(a);
     } else {
         layout((char*)workspace, cfg->n_trees, cfg->horizon, cfg->C, true, a.st);
-        sparse_sampling_kernel<SHighwayEnv><<<lane_grid(cfg->n_trees, SHighwayEnv::GROUP), 128, 0, stream>>>(a);
+        sparse_sampling_kernel<SHighwayEnv><<<lane_grid<SHighwayEnv>(cfg->n_trees), 128, 0, stream>>>(a);
     }
     B2_CUDA_CHECK(cudaGetLastError());
     return B2_OK;

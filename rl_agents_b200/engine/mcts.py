@@ -6,8 +6,7 @@ its env copies, so those take the live env's generator words (`env_words`), whic
 import numpy as np
 
 from rl_agents_b200 import _lib
-from rl_agents_b200.engine.tables import (FiniteTables, SampledFiniteTables, gamma_tables, preference_tables,
-                                          uniform_cdf_table)
+from rl_agents_b200.engine.tables import finite_model, gamma_tables, preference_tables, uniform_cdf_table
 from rl_agents_b200.engine.tree_engine import TreeEngine, decode_action
 
 POLICIES = {"random_available": 0, "random": 1, "preference": 2}
@@ -92,21 +91,16 @@ class MCTSEngine(TreeEngine):
         gp, _ = gamma_tables(gamma, self.horizon + 1)
         self.gamma_pow = torch.as_tensor(gp, device=self.device)
         self.cdf = torch.as_tensor(uniform_cdf_table(self.n_actions), device=self.device)
-        self.sampled = env_kind == _lib.ENV_FINITE and mdp.mode != "deterministic"
-        self.tables = None
+        self.sampled, self.tables, finite_mdp = finite_model(env_kind, mdp, self.device)
         if self.sampled:
-            self.tables = SampledFiniteTables(mdp, self.device)
             self.env_rng = torch.empty((self.n_trees, _lib.PCG64_STATE_WORDS), dtype=torch.int64, device=self.device)
-        elif env_kind == _lib.ENV_FINITE:
-            self.tables = FiniteTables(mdp, self.device)
         self.tree = _lib.MCTSTree(*self._alloc_tree(_lib.MCTS_TREE_FIELDS, self.capacity))
         self.pref_prior = torch.as_tensor(preference_tables(self.n_actions, prior_ratio)[0], device=self.device)
         self.pref_cdf = torch.as_tensor(preference_tables(self.n_actions, rollout_ratio)[1], device=self.device)
         self.cfg = _lib.MCTSConfig(env_kind, self.n_trees, self.n_actions, self.episodes, self.horizon, self.capacity,
                                    rollout_id, prior_id, float(temperature),
                                    self.gamma_pow.data_ptr(), self.cdf.data_ptr(),
-                                   self.tables.struct() if self.tables and not self.sampled else _lib.FiniteMDP(),
-                                   prior_action, rollout_action, self.pref_prior.data_ptr(), self.pref_cdf.data_ptr(), None)
+                                   finite_mdp, prior_action, rollout_action, self.pref_prior.data_ptr(), self.pref_cdf.data_ptr(), None)
         self.resume = torch.zeros(self.n_trees, dtype=torch.int32, device=self.device)
         self.plan_buf = torch.empty((self.n_trees, max(self.horizon, 1)), dtype=torch.int8, device=self.device)
 
@@ -182,14 +176,10 @@ class MCTSWaveEngine(object):
         self.capacity = 1 + self.episodes * self.n_actions
         gp, _ = gamma_tables(gamma, self.horizon + 1)
         self.gamma_pow = torch.as_tensor(gp, device=self.device)
-        self.sampled = env_kind == _lib.ENV_FINITE and mdp.mode != "deterministic"
-        self.tables = None
+        self.sampled, self.tables, finite_mdp = finite_model(env_kind, mdp, self.device)
         if self.sampled:
-            self.tables = SampledFiniteTables(mdp, self.device)
             self.env_rng = torch.empty(_lib.PCG64_STATE_WORDS, dtype=torch.int64, device=self.device)
             self.rejected = torch.empty(2, dtype=torch.int32, device=self.device)
-        elif env_kind == _lib.ENV_FINITE:
-            self.tables = FiniteTables(mdp, self.device)
         i32 = torch.int32
         self.parent = torch.empty(self.capacity, dtype=i32, device=self.device)
         self.first_child = torch.empty(self.capacity, dtype=i32, device=self.device)
@@ -199,8 +189,7 @@ class MCTSWaveEngine(object):
         self.value = torch.empty(self.capacity, dtype=torch.float64, device=self.device)
         self.cfg = _lib.MCTSWaveConfig(env_kind, self.n_actions, self.episodes, self.horizon, self.capacity, self.width,
                                        0, 0, float(temperature), 0, self.gamma_pow.data_ptr(),
-                                       self.tables.struct() if self.tables and not self.sampled else _lib.FiniteMDP(),
-                                       int(max_ctas), 0)
+                                       finite_mdp, int(max_ctas), 0)
         self.tree = _lib.MCTSWaveTree(*[t.data_ptr() for t in (self.parent, self.first_child, self.count, self.meta,
                                                                self.vsum, self.value)])
         ws = self.lib.b2_mcts_wave_workspace_bytes(self.cfg)

@@ -5,7 +5,7 @@ b2_mdp_gape_plan_sampled on SampledFiniteTables, where chance nodes observe seve
 import numpy as np
 
 from rl_agents_b200 import _lib
-from rl_agents_b200.engine.tables import FiniteTables, SampledFiniteTables
+from rl_agents_b200.engine.tables import finite_model
 from rl_agents_b200.engine.tree_engine import TreeEngine, decode_action
 
 
@@ -47,20 +47,17 @@ class MDPGapEEngine(TreeEngine):
         self.thresholds = table(upper_bound["threshold"])
         self.transition_thresholds = table(upper_bound["transition_threshold"])
         self.init_upper = torch.as_tensor(init_upper, device=self.device)
-        self.sampled = env_kind == _lib.ENV_FINITE and mdp.mode != "deterministic"
-        self.tables, self.keys = None, None
+        self.sampled, self.tables, finite_mdp = finite_model(env_kind, mdp, self.device)
+        self.keys = None
         if self.sampled:
-            self.tables = SampledFiniteTables(mdp, self.device)
             self.terminal = self.tables.terminal
             self.keys = torch.empty((self.n_trees, self.capacity), dtype=torch.int32, device=self.device)
-        elif env_kind == _lib.ENV_FINITE:
-            self.tables = FiniteTables(mdp, self.device)
         self.tree = _lib.MDPGapETree(*self._alloc_tree(_lib.MDP_GAPE_TREE_FIELDS, self.capacity))
         self.cfg = _lib.MDPGapEConfig(env_kind, self.n_trees, self.n_actions, self.episodes, self.horizon,
                                       self.capacity, self.n_next, 1 if continuation_type == "uniform" else 0, gamma,
                                       float(accuracy), self.thresholds.data_ptr(),
                                       self.transition_thresholds.data_ptr(), self.init_upper.data_ptr(),
-                                      self.tables.struct() if self.tables and not self.sampled else _lib.FiniteMDP())
+                                      finite_mdp)
         self.plan_buf = torch.empty(self.n_trees, dtype=torch.int8, device=self.device)
 
     def plan(self, root_states, rng_words):

@@ -8,7 +8,7 @@ import logging
 import numpy as np
 
 from rl_agents_b200 import _lib
-from rl_agents_b200.engine.tables import FiniteTables, SampledFiniteTables
+from rl_agents_b200.engine.tables import finite_model
 from rl_agents_b200.engine.tree_engine import TreeEngine, decode_action
 
 logger = logging.getLogger(__name__)
@@ -46,18 +46,14 @@ class OLOPEngine(TreeEngine):
         self.init_upper = torch.as_tensor(init_upper, device=self.device)
         self.thresholds = torch.as_tensor(thresholds_for(upper_bound, self.episodes) if self.kl
                                           else np.zeros(max(self.episodes, 1)), device=self.device)
-        self.sampled = env_kind == _lib.ENV_FINITE and mdp.mode != "deterministic"
-        self.tables = None
+        self.sampled, self.tables, finite_mdp = finite_model(env_kind, mdp, self.device)
         if self.sampled:
-            self.tables = SampledFiniteTables(mdp, self.device)
             self.terminal = self.tables.terminal
-        elif env_kind == _lib.ENV_FINITE:
-            self.tables = FiniteTables(mdp, self.device)
         self.tree = _lib.OLOPTree(*self._alloc_tree(_lib.OLOP_TREE_FIELDS, self.capacity))
         self.cfg = _lib.OLOPConfig(env_kind, self.n_trees, self.n_actions, self.episodes, self.horizon, self.capacity,
                                    1 if self.kl else 0, 1 if continuation_type == "uniform" else 0, gamma,
                                    self.thresholds.data_ptr(), self.init_upper.data_ptr(),
-                                   self.tables.struct() if self.tables and not self.sampled else _lib.FiniteMDP())
+                                   finite_mdp)
         self.plan_buf = torch.empty((self.n_trees, max(self.horizon, 1)), dtype=torch.int8, device=self.device)
 
     def plan(self, root_states, rng_words):

@@ -125,6 +125,20 @@ class SampledFiniteTables(object):
                                      self.next.data_ptr(), self.reward.data_ptr(), self.row_ok.data_ptr())
 
 
+def finite_model(env_kind, mdp, device):
+    """-> (sampled, tables, the b2_finite_mdp a planner config carries) of an engine on env_kind: a finite MDP in
+    mode "deterministic" gets FiniteTables, whose struct the config carries; in any other mode SampledFiniteTables,
+    passed to the *_sampled entry point, and the config carries an empty struct, as on the other env kinds, which get no
+    tables."""
+    from rl_agents_b200 import _lib
+    if env_kind != _lib.ENV_FINITE:
+        return False, None, _lib.FiniteMDP()
+    if mdp.mode == "deterministic":
+        tables = FiniteTables(mdp, device)
+        return False, tables, tables.struct()
+    return True, SampledFiniteTables(mdp, device), _lib.FiniteMDP()
+
+
 class FiniteTables(object):
     """Device copy of a deterministic finite MDP (int32 transitions)."""
 
