@@ -106,6 +106,38 @@ int b2_selftest_highway_step_groups(const int32_t* states, const int32_t* action
                                     int32_t* trace, float* reward, int32_t* flags, int32_t n_scenes,
                                     int32_t max_steps, void* stream);
 
+/* Self-tests of the device primitives the planners share (tests/test_gpu_device_primitives.py), one thread per
+ * stream or case, each calling the planners' own inline functions. */
+
+/* numpy's PCG64 (pcg64.cuh): stream s loads words [n_streams, 6] and runs ops[s, 0 .. n_ops-1] with args:
+ * 0 next64, 1 next32, 2 random (out = the double's bits), 3 integers(arg) (Generator.integers(0, arg), 1 <= arg < 2^32),
+ * 4 skip32(arg) and 5 seed_from(arg) (both: out = the low 64 bits of the LCG state after the op), any other code: no op,
+ * out left as it was.  out [n_streams, n_ops]; words_out [n_streams, 6] the words after the last op. */
+int b2_selftest_pcg64(const uint64_t* words, const int32_t* ops, const uint64_t* args, uint64_t* out,
+                      uint64_t* words_out, int32_t n_streams, int32_t n_ops, void* stream);
+
+/* kl_bound.cuh: kl[i] = bernoulli_kl(p[i], q[i]) for i < n_kl; bound[i] = kl_bound(sum[i], count[i], threshold[i],
+ * lower[i] != 0) for i < n_bound.  Either part may be empty. */
+int b2_selftest_kl(const double* p, const double* q, int32_t n_kl, double* kl, const double* sum,
+                   const int32_t* count, const double* threshold, const int32_t* lower, int32_t n_bound, double* bound,
+                   void* stream);
+
+/* lane_env.cuh: k[i] = searchsorted_right(cdf + u_row[i] * n_next, n_next, u[i]) for i < n_u (cdf rows of n_next
+ * entries); and for i < n_steps, sampled_next(*mdp, rows[i], draw[i] != 0, g) with g loaded from words [n_steps, 6]:
+ * next [n_steps] and the words afterwards, words_out [n_steps, 6].  Either part may be empty. */
+int b2_selftest_sampled_next(const double* cdf, int32_t n_next, const double* u, const int32_t* u_row, int32_t n_u,
+                             int32_t* k, const struct b2_finite_mdp_sampled* mdp, const int64_t* rows,
+                             const int32_t* draw, const uint64_t* words, int32_t n_steps, int32_t* next,
+                             uint64_t* words_out, void* stream);
+
+/* mdp_gape.cu's backup expectations: case i is a chance node whose children 0 .. K[i]-1 sit at i * max_k + j of
+ * f, neg_f (= -f), counts and zeros (max_k * n_cases zeros), valued with gamma = 1.  n[i] == 0: gape_expectation (one
+ * observed child, child 0, with p_hat qp[i]); n[i] >= 1: gape_expectation_kl with children 0 .. n[i]-1 observed,
+ * p_hat = counts / cnt[i].  out [n_cases, 2]: the upper side (values f), then the lower side (values -f). */
+int b2_selftest_gape_expectation(const double* f, const double* neg_f, const int32_t* counts, const double* zeros,
+                                 int32_t max_k, const int32_t* K, const int32_t* n, const int32_t* cnt,
+                                 const double* qp, const double* c, int32_t n_cases, double* out, void* stream);
+
 /* ------------------------------------------------------------------------
  * Value iteration -- rl_agents/agents/dynamic_programming/value_iteration.py
  * ---------------------------------------------------------------------- */

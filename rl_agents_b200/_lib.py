@@ -220,6 +220,12 @@ EXPORTS = {
     "b2_intersection_step": (c_int, [c_void_p] * 5 + [c_int32, c_void_p]),
     "b2_selftest_const_division": (c_int, [c_void_p, c_void_p]),
     "b2_selftest_highway_step_groups": (c_int, [c_void_p] * 6 + [c_int32, c_int32, c_void_p]),
+    "b2_selftest_pcg64": (c_int, [c_void_p] * 5 + [c_int32, c_int32, c_void_p]),
+    "b2_selftest_kl": (c_int, [c_void_p, c_void_p, c_int32, c_void_p] + [c_void_p] * 4 + [c_int32, c_void_p, c_void_p]),
+    "b2_selftest_sampled_next": (c_int, [c_void_p, c_int32, c_void_p, c_void_p, c_int32, c_void_p,
+                                         ctypes.POINTER(FiniteMDPSampled)] + [c_void_p] * 3 + [c_int32] +
+                                 [c_void_p] * 3),
+    "b2_selftest_gape_expectation": (c_int, [c_void_p] * 4 + [c_int32] + [c_void_p] * 5 + [c_int32, c_void_p, c_void_p]),
     "b2_highway_step": (c_int, [c_void_p] * 5 + [c_int32, c_void_p]),
     "b2_highway_ttc_vi": (c_int, [c_void_p, c_int32, c_double, c_int32, c_double, c_double] + [c_void_p] * 5),
     "b2_vi_sweep": (c_int, [ctypes.POINTER(VIProblem)] + [c_void_p] * 5 + [c_int32, c_void_p]),

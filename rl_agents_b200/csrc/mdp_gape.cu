@@ -408,6 +408,19 @@ __global__ void __launch_bounds__(128, 8) mdp_gape_kernel(GapeArgs a) {
     }
 }
 
+// b2_selftest_gape_expectation: case i is chance node 0 of a tree whose children fc = 0 .. K-1 hold mu_ucb = f,
+// mu_lcb = -f, upper = lower = 0 and integer counts, with gamma = 1, so that value() is mu_ucb or mu_lcb exactly.
+__global__ void gape_expectation_selftest_kernel(b2_mdp_gape_tree tr, int max_k, const int32_t* K, const int32_t* n,
+                                                 const int32_t* cnt, const double* qp, const double* c, int n_cases,
+                                                 double* out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_cases) return;
+    const int64_t nb = (int64_t)i * max_k;
+    for (int side = 0; side < 2; ++side)
+        out[2 * i + side] = n[i] == 0 ? gape_expectation(tr, nb, 0, K[i], side == 0, 1.0, qp[i], c[i])
+                                      : gape_expectation_kl(tr, nb, 0, K[i], n[i], side == 0, 1.0, cnt[i], c[i]);
+}
+
 }  // namespace
 }  // namespace b2
 
@@ -455,6 +468,23 @@ extern "C" int b2_mdp_gape_plan_sampled(const b2_mdp_gape_config* cfg, const b2_
     a.cfg = *cfg; a.tree = *tree; a.root_states = root_states; a.rng = rng; a.plan = plan; a.result = result;
     a.keys = keys; a.model = LaneModel{b2_finite_mdp{}, *mdp, terminal, env_draws};
     mdp_gape_kernel<SampledFiniteEnv><<<lane_grid<SampledFiniteEnv>(cfg->n_trees), 128, 0, stream>>>(a);
+    B2_CUDA_CHECK(cudaGetLastError());
+    return B2_OK;
+}
+
+extern "C" int b2_selftest_gape_expectation(const double* f, const double* neg_f, const int32_t* counts,
+                                            const double* zeros, int32_t max_k, const int32_t* K, const int32_t* n,
+                                            const int32_t* cnt, const double* qp, const double* c, int32_t n_cases,
+                                            double* out, void* stream) {
+    B2_REQUIRE(f && neg_f && counts && zeros && K && n && cnt && qp && c && out, "null pointer");
+    B2_REQUIRE(n_cases > 0 && max_k >= 1, "empty batch");
+    b2_mdp_gape_tree tr{};
+    tr.count = const_cast<int32_t*>(counts);
+    tr.mu_ucb = const_cast<double*>(f);
+    tr.mu_lcb = const_cast<double*>(neg_f);
+    tr.upper = tr.lower = const_cast<double*>(zeros);
+    gape_expectation_selftest_kernel<<<(n_cases + 127) / 128, 128, 0, (cudaStream_t)stream>>>(tr, max_k, K, n, cnt, qp,
+                                                                                              c, n_cases, out);
     B2_CUDA_CHECK(cudaGetLastError());
     return B2_OK;
 }
