@@ -87,4 +87,11 @@ __device__ __forceinline__ double warp_max_f64(double v) {
 __device__ __forceinline__ double np_max(double m, double x) { return (x > m || isnan(x)) ? x : m; }
 __device__ __forceinline__ double np_min(double m, double x) { return (x < m || isnan(x)) ? x : m; }
 
+// numpy.isclose(a, b, rtol, atol) as numpy >= 2 states it: (|a - b| <= atol + rtol * |b| and b finite) or a == b.  Equal
+// infinities are close, NaN is close to nothing, and so are equal finite values even when atol + rtol * |b| < 0 (the
+// value-iteration sweeps' "early exit off" setting rtol = 0, atol = -1 still stops at an exact fixed point).
+__device__ __forceinline__ bool np_isclose(double a, double b, double rtol, double atol) {
+    return (fabs(a - b) <= atol + rtol * fabs(b) && isfinite(b)) || a == b;
+}
+
 }  // namespace b2

@@ -67,12 +67,6 @@ __device__ __forceinline__ double np_pairwise_sum(Load a, int lo, int n) {
     return np_pairwise_sum_big(a, lo, n);
 }
 
-__device__ __forceinline__ bool np_isclose(double a, double b, double rtol, double atol) {
-    // numpy.isclose: finite -> |a-b| <= atol + rtol*|b| ; otherwise a == b
-    if (isfinite(a) && isfinite(b)) return fabs(a - b) <= atol + rtol * fabs(b);
-    return a == b;
-}
-
 struct SweepArgs {
     const double* P;       // sparse/stochastic probabilities (slab-local)
     const int32_t* N;      // sparse successors or deterministic transition

@@ -16,11 +16,6 @@
 
 namespace b2 {
 
-__device__ __forceinline__ bool p2p_isclose(double a, double b, double rtol, double atol) {
-    if (isfinite(a) && isfinite(b)) return fabs(a - b) <= atol + rtol * fabs(b);
-    return a == b;
-}
-
 __device__ __forceinline__ int ld_acquire_sys(const int32_t* p) {
     int v;
     asm volatile("ld.acquire.sys.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
@@ -124,7 +119,7 @@ __global__ void __launch_bounds__(256) vi_sweep_row_p2p_kernel(P2PSweep g) {
                 }
                 if (g.term[qi / A]) nv = 0.0;
                 q = __ldcs(g.R + qi) + g.gamma * nv;
-                if (!p2p_isclose(__ldcs(g.q_old + qi), q, g.rtol, g.atol)) bad++;
+                if (!np_isclose(__ldcs(g.q_old + qi), q, g.rtol, g.atol)) bad++;
                 __stcs(g.q_new + qi, q);
             }
             double m = q;

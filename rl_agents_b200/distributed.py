@@ -61,6 +61,66 @@ def allgather_slabs(full, n, group=None):
     return full
 
 
+def p2p_layout(n_states, world, max_iterations):
+    """Byte offsets into the peer-memory buffer every rank of DistributedVI(exchange="p2p") holds, each region
+    256-byte aligned: the V ping-pong pair "v" [2 x S f64], "flags" [G i32] (entry r = sweeps rank r has published),
+    "parts" [T x G i32] (row k, column r = rank r's violation count at sweep k), then the rank-local scratch that no
+    peer reads, "viol_local" [T i32], "done" [T u32] and "status" (one i32); "nbytes" is the whole buffer."""
+    S, G, T = int(n_states), int(world), int(max_iterations)
+    al = lambda n: (n + 255) // 256 * 256
+    v = (0, al(S * 8))
+    flags = v[1] + al(S * 8)
+    parts = flags + al(G * 4)
+    viol_local = parts + al(T * G * 4)
+    done = viol_local + al(T * 4)
+    status = done + al(T * 4)
+    return dict(v=v, flags=flags, parts=parts, viol_local=viol_local, done=done, status=status, nbytes=status + 256)
+
+
+def p2p_exchange(layout, bases, rank):
+    """The b2_vi_p2p of `rank` in a world of len(bases) ranks whose buffers (p2p_layout) start at the device addresses
+    bases[r], as this process addresses them: V, flags and parts name every rank's buffer, the scratch only its own."""
+    from rl_agents_b200 import _lib
+    x = _lib.VIP2P()
+    x.world, x.rank = len(bases), rank
+    for r, base in enumerate(bases):
+        x.v[0][r], x.v[1][r] = base + layout["v"][0], base + layout["v"][1]
+        x.flags[r], x.parts[r] = base + layout["flags"], base + layout["parts"]
+    x.viol_local = bases[rank] + layout["viol_local"]
+    x.done = bases[rank] + layout["done"]
+    x.status = bases[rank] + layout["status"]
+    return x
+
+
+def p2p_result(parts):
+    """(k, sweeps) from the [iterations, G] table of per-slab violation counts: the first sweep k whose summed count
+    is zero met np.allclose, so iterate k (the OLD one) is returned after k + 1 sweeps; with none, the last iterate."""
+    zero = np.nonzero(np.asarray(parts).sum(axis=1) == 0)[0]
+    if zero.size:
+        return int(zero[0]), int(zero[0]) + 1
+    return len(parts), len(parts)
+
+
+P2P_MODES = ("sparse", "deterministic")
+
+
+def check_p2p_problem(mode, n_states, n_actions, n_next, world):
+    """ValueError for every problem b2_vi_sweep_p2p refuses whatever the rank: the mode, A a power of two <= 32, B in
+    {1, 2, 4, 8}, and a state count that leaves some rank an empty slab.  Every rank raises alike, before any rank
+    allocates or waits on a peer."""
+    from rl_agents_b200 import _lib
+    if world > _lib.MAX_PEERS:
+        raise ValueError("p2p exchange supports up to %d ranks" % _lib.MAX_PEERS)
+    if mode not in P2P_MODES:
+        raise ValueError("p2p exchange supports the sparse and deterministic modes, not %r" % (mode,))
+    if n_actions < 1 or n_actions > 32 or n_actions & (n_actions - 1):
+        raise ValueError("p2p exchange needs a number of actions that is a power of two <= 32 (got %d)" % n_actions)
+    if n_next not in (1, 2, 4, 8):
+        raise ValueError("p2p exchange needs 1, 2, 4 or 8 successors per action (got %d)" % n_next)
+    if n_states < world:
+        raise ValueError("p2p exchange needs a state for every rank (%d states, %d ranks)" % (n_states, world))
+
+
 class PeerBuffer(object):
     """A device buffer of `nbytes` per rank that every rank of the group can address (CUDA IPC over
     NVLink / NVSwitch): `ptrs[r]` is the address of rank r's buffer in THIS process (ptrs[rank] is the
@@ -148,36 +208,31 @@ class DistributedVI(object):
             slab = (np.asarray(transition)[b:e], np.asarray(reward)[b:e], np.asarray(terminal)[b:e],
                     None if nxt is None else np.asarray(nxt)[b:e])
         self.n_states = S
+        if exchange == "p2p":
+            n_next = 1 if mode != "sparse" else (0 if nxt is None else int(nxt.shape[-1]))
+            check_p2p_problem(mode, S, int(reward.shape[-1]), n_next, self.world)
+        elif exchange != "nccl":
+            raise ValueError("exchange must be 'nccl' or 'p2p'")
         self.engine = VIEngine(mode, slab[0], slab[1], slab[2], nxt=slab[3], gamma=gamma, device=device,
                                row_begin=b, row_end=e, n_states=S, rtol=rtol, atol=atol)
         if exchange == "p2p":
             self._setup_p2p()
-        elif exchange != "nccl":
-            raise ValueError("exchange must be 'nccl' or 'p2p'")
 
     # ------------------------------------------------------------------ fused exchange over peer memory
     def _setup_p2p(self):
-        from rl_agents_b200 import _lib
-        if self.world > _lib.MAX_PEERS:
-            raise ValueError("p2p exchange supports up to %d ranks" % _lib.MAX_PEERS)
-        S, G, T = self.n_states, self.world, self.max_iterations
-        al = lambda n: (n + 255) // 256 * 256
-        self._off_v = [0, al(S * 8)]
-        self._off_flags = self._off_v[1] + al(S * 8)
-        self._off_parts = self._off_flags + al(G * 4)
-        self._off_local = self._off_parts + al(T * G * 4)        # viol_local [T] + done [T]: never read by peers
-        self._bytes = self._off_local + al(T * 4) + al(T * 4) + 256
-        self.peer = PeerBuffer(self._bytes, self.group)
-        x = _lib.VIP2P()
-        x.world, x.rank = G, self.rank
-        for r in range(G):
-            base = self.peer.ptrs[r]
-            x.v[0][r], x.v[1][r] = base + self._off_v[0], base + self._off_v[1]
-            x.flags[r], x.parts[r] = base + self._off_flags, base + self._off_parts
-        x.viol_local = self.peer.local + self._off_local
-        x.done = self.peer.local + self._off_local + al(T * 4)
-        x.status = self.peer.local + self._off_local + 2 * al(T * 4)
-        self._x = x
+        # b2_vi_sweep_p2p also refuses successor / probability tables that are not 16-byte aligned (a caller's device
+        # slab at an odd element offset).  Only this rank can see that, and a rank that refused its first sweep would
+        # leave its peers waiting for its arrival flag: such a slab is copied into a fresh (aligned) allocation instead.
+        eng = self.engine
+        for name in ("transition", "next"):              # VIEngine's tensors and b2_vi_problem's fields alike
+            t = getattr(eng, name)
+            if t is not None and t.data_ptr() % 16:
+                t = t.clone()
+                setattr(eng, name, t)
+                setattr(eng.problem, name, t.data_ptr())
+        self._layout = p2p_layout(self.n_states, self.world, self.max_iterations)
+        self.peer = PeerBuffer(self._layout["nbytes"], self.group)
+        self._x = p2p_exchange(self._layout, self.peer.ptrs, self.rank)
 
     def _solve_p2p(self, iterations):
         import ctypes
@@ -189,7 +244,7 @@ class DistributedVI(object):
         stream = _lib.current_stream()
         for q in eng.q:
             q.zero_()
-        _lib.check(lib.b2_p2p_memset(ctypes.c_void_p(self.peer.local), 0, self._bytes, stream))
+        _lib.check(lib.b2_p2p_memset(ctypes.c_void_p(self.peer.local), 0, self._layout["nbytes"], stream))
         torch.cuda.synchronize()
         self.dist.barrier(group=self.group)      # every rank's flags are zero before anybody publishes
         for k in range(iterations):
@@ -197,22 +252,18 @@ class DistributedVI(object):
                                            k, stream))
         parts = np.zeros((iterations, self.world), dtype=np.int32)
         _lib.check(lib.b2_p2p_read(parts.ctypes.data_as(ctypes.c_void_p),
-                                   ctypes.c_void_p(self.peer.local + self._off_parts), parts.nbytes, stream))
+                                   ctypes.c_void_p(self.peer.local + self._layout["parts"]), parts.nbytes, stream))
         # a rank reads its own table only after ITS last kernel retired; peers publish their last entry
         # when THEIR last kernel retires: wait for everybody before trusting the last row
         self.dist.barrier(group=self.group)
         _lib.check(lib.b2_p2p_read(parts.ctypes.data_as(ctypes.c_void_p),
-                                   ctypes.c_void_p(self.peer.local + self._off_parts), parts.nbytes, stream))
+                                   ctypes.c_void_p(self.peer.local + self._layout["parts"]), parts.nbytes, stream))
         status = np.zeros(1, dtype=np.int32)
         _lib.check(lib.b2_p2p_read(status.ctypes.data_as(ctypes.c_void_p), ctypes.c_void_p(self._x.status), 4, stream))
         if int(status[0]) != 0:
             raise _lib.B2Error("p2p value iteration: a peer's arrival flag timed out (rank %d)" % self.rank)
-        viol = parts.sum(axis=1)
-        zero = np.nonzero(viol == 0)[0]
-        if zero.size:
-            k = int(zero[0])
-            return eng.q[k & 1], k + 1
-        return eng.q[iterations & 1], int(iterations)
+        k, sweeps = p2p_result(parts)
+        return eng.q[k & 1], sweeps
 
     def v_slab(self, iterations_done):
         """(p2p) this rank's copy of the full V after `iterations_done` sweeps, as a host array."""
@@ -220,7 +271,7 @@ class DistributedVI(object):
         from rl_agents_b200 import _lib
         out = np.zeros(self.n_states, dtype=np.float64)
         _lib.check(self.peer.lib.b2_p2p_read(out.ctypes.data_as(ctypes.c_void_p),
-                                             ctypes.c_void_p(self.peer.local + self._off_v[iterations_done & 1]),
+                                             ctypes.c_void_p(self.peer.local + self._layout["v"][iterations_done & 1]),
                                              out.nbytes, _lib.current_stream()))
         return out
 
