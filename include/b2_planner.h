@@ -92,6 +92,21 @@ int b2_highway_ttc_vi(const int32_t* states, int32_t n_envs, double gamma, int32
 int b2_intersection_step(int32_t* states, const int32_t* actions, float* reward, int32_t* flags,
                          int32_t* avail_mask, int32_t n_envs, void* stream);
 
+/* FiniteMDPEnv.step on a batch of n episodes of one finite MDP in any mode (the `finite_mdp` package's MDP.step),
+ * one thread per episode, with the sampled planners' own step (lane_env.cuh, SampledFiniteEnv::step).  For every
+ * episode i with alive[i] != 0, from s = states[i] and a = actions[i]: reward[i] = reward[s, a]; flags[i] bit0 =
+ * terminal[s] (done is read on the state the action is taken in); states[i] = next[s, a, k] with k = 0 when
+ * env_draws == 0 ("deterministic"), else k = Generator.choice(p.size, p=p[s, a]) of the episode's env generator,
+ * env_rng [n, 6] words (pcg64_words), advanced in place; bad_row[i] = -1.  A row Generator.choice rejects (row_ok 0)
+ * leaves states[i] and the generator unchanged, sets reward[i] = 0, flags[i] = 0 and reports the row s * A + a in
+ * bad_row[i].  Episodes with alive[i] == 0 are not touched.  env_rng may be NULL when env_draws == 0.
+ * The states and actions of the live episodes are checked on the device first, and the call synchronises `stream`
+ * to read that check: a state outside [0, n_states) or an action outside [0, n_actions) steps no episode and returns
+ * B2_ERR_INVALID. */
+int b2_finite_step(const struct b2_finite_mdp_sampled* mdp, const uint8_t* terminal, int32_t env_draws,
+                   int32_t* states, const int32_t* actions, const uint8_t* alive, uint64_t* env_rng, double* reward,
+                   int32_t* flags, int32_t* bad_row, int32_t n, void* stream);
+
 /* Self-test (tests/test_gpu_engines.py): the HighwayLite kernel divides by two constants of the spec with a
  * 3-instruction sequence instead of the full IEEE division; this compares both, exhaustively over every fp32
  * mantissa, both signs and exponents -60..60, and writes the number of differing results (must be 0). */

@@ -227,6 +227,8 @@ EXPORTS = {
                                  [c_void_p] * 3),
     "b2_selftest_gape_expectation": (c_int, [c_void_p] * 4 + [c_int32] + [c_void_p] * 5 + [c_int32, c_void_p, c_void_p]),
     "b2_highway_step": (c_int, [c_void_p] * 5 + [c_int32, c_void_p]),
+    "b2_finite_step": (c_int, [ctypes.POINTER(FiniteMDPSampled), c_void_p, c_int32] + [c_void_p] * 7
+                       + [c_int32, c_void_p]),
     "b2_highway_ttc_vi": (c_int, [c_void_p, c_int32, c_double, c_int32, c_double, c_double] + [c_void_p] * 5),
     "b2_vi_sweep": (c_int, [ctypes.POINTER(VIProblem)] + [c_void_p] * 5 + [c_int32, c_void_p]),
     "b2_vi_solve": (c_int, [ctypes.POINTER(VIProblem)] + [c_void_p] * 5 + [c_int32, c_void_p]),

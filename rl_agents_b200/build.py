@@ -10,7 +10,7 @@ LIB = os.path.join(CSRC, "libb2planner.so")
 STAMP = LIB + ".cmd"          # signature() of the build that made the library
 SOURCES = ["common.cu", "vi.cu", "vi_p2p.cu", "opd.cu", "opd_wave.cu", "gbop.cu", "mcts.cu", "mcts_wave.cu", "olop.cu",
            "mdp_gape.cu", "brue.cu", "sparse_sampling.cu", "sparse_sampling_levels.cu",
-           "mcts_dpw.cu", "platypoos.cu", "ttc_vi.cu", "selftest.cu", "host_api.cu"]
+           "mcts_dpw.cu", "platypoos.cu", "ttc_vi.cu", "finite_step.cu", "selftest.cu", "host_api.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     # parity: every fp op is a single IEEE operation (no FMA contraction), IEEE div/sqrt, no FTZ

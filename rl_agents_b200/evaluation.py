@@ -1,4 +1,5 @@
-"""Batched closed-loop evaluation of the planners on HighwayLite (and of MCTS and OLOP on IntersectionLite): the
+"""Batched closed-loop evaluation of the planners on HighwayLite (of MCTS and OLOP on IntersectionLite, and of every
+planner on finite MDPs, stepped by b2_finite_step): the
 working version of the reference's disabled budget-sweep harness (scripts/planners_evaluation.py:287-289, SURVEY 8f
 rank 4) in the shape the GPU wants -- all episodes advance in lock-step, every decision step is
 ONE batched plan() launch over all live episodes and ONE batched env transition."""
@@ -11,6 +12,10 @@ from rl_agents_b200.envs import highway_lite, intersection_lite
 
 # planners with an IntersectionLite model (b2_mcts_plan, b2_olop_plan)
 INTERSECTION_PLANNERS = ("mcts", "olop")
+# GBOP-T (StateAwarePlannerAgent) and GBOP-D (GraphBasedPlannerAgent): deterministic finite MDPs only
+GBOP_PLANNERS = ("gbop", "gbopd")
+# planners whose agents refuse a finite MDP in mode "stochastic" or "sparse"
+DETERMINISTIC_ONLY_PLANNERS = ("opd", "brue") + GBOP_PLANNERS
 
 
 def _np_random(seed):
@@ -28,7 +33,14 @@ def run_batched_episodes(planner, seeds, budget, gamma, max_steps=40, device="cu
     env: "highway" (HighwayLite, every planner) or "intersection" (IntersectionLite scenes of
     envs.intersection_lite.make_scene stepped by b2_intersection_step, "mcts" and "olop" only; an episode also ends
     when the ego arrives or at the env's duration).  `crashed` is the ego's crash flag.
+    env "finite": closed-loop episodes on a finite MDP, see run_finite_episodes (keywords `mdp`, `start_states`,
+    `env_seed`).
     Returns dict(returns, lengths, crashed, decision_ms)."""
+    if env == "finite":
+        return run_finite_episodes(planner, len(seeds), budget, gamma, max_steps=max_steps, device=device,
+                                   planner_seed=planner_seed, **kw)
+    if planner in GBOP_PLANNERS and env in ("highway", "intersection"):
+        raise NotImplementedError("%r aggregates nodes by state id: it runs on finite MDPs only" % planner)
     import torch
     from rl_agents_b200.engine.mcts import MCTSEngine, pcg64_words, set_pcg64_words
     from rl_agents_b200.engine.olop import OLOPEngine
@@ -146,3 +158,191 @@ def run_batched_episodes(planner, seeds, budget, gamma, max_steps=40, device="cu
         alive &= ~done
     return {"returns": returns, "lengths": lengths, "crashed": crashed, "actions": np.array(actions_log).T,
             "decision_ms": 1e3 * t_plan / max(len(actions_log), 1), "n": n}
+
+
+def _completed_config(agent_cls, planner_cls, kw, budget, gamma):
+    """The planner config of agent_cls(env, dict(kw, budget=budget, gamma=gamma)): the agent's defaults updated with
+    the keywords, then the planner's defaults updated with that."""
+    cfg = agent_cls.default_config()
+    agent_cls.rec_update(cfg, dict(kw, budget=budget, gamma=gamma))
+    pcfg = planner_cls.default_config()
+    planner_cls.rec_update(pcfg, cfg)
+    return pcfg
+
+
+def _finite_engine_factory(planner, mdp, n_actions, budget, gamma, kw, dev):
+    """-> make(n_trees): the engine of `planner` on the finite MDP `mdp` with its drop-in agent's completed config."""
+    from rl_agents_b200.agents.tree_search.mcts import MCTS, MCTSAgent, allocation
+    E, A = _lib.ENV_FINITE, n_actions
+    if planner == "opd":
+        from rl_agents_b200.agents.tree_search.deterministic import (DeterministicPlannerAgent,
+                                                                     OptimisticDeterministicPlanner)
+        from rl_agents_b200.engine.opd import OPDEngine
+        c = _completed_config(DeterministicPlannerAgent, OptimisticDeterministicPlanner, kw, budget, gamma)
+        return lambda m: OPDEngine(E, m, A, budget, gamma, c.get("terminal_reward", 0), mdp=mdp, device=dev,
+                                   keys_in_smem=c.get("keys_in_smem", True))
+    if planner == "gbop":
+        from rl_agents_b200.agents.tree_search.state_aware import StateAwarePlanner, StateAwarePlannerAgent
+        from rl_agents_b200.engine.gbop import GBOPEngine
+        c = _completed_config(StateAwarePlannerAgent, StateAwarePlanner, kw, budget, gamma)
+        return lambda m: GBOPEngine(m, A, budget, gamma, mdp, c.get("terminal_reward", 0), c["backup_aggregated_nodes"],
+                                    c["prune_suboptimal_leaves"], c["accuracy"], device=dev)
+    if planner == "gbopd":
+        from rl_agents_b200.agents.tree_search.graph_based import GraphBasedPlanner, GraphBasedPlannerAgent
+        from rl_agents_b200.engine.gbop import GBOPDEngine
+        c = _completed_config(GraphBasedPlannerAgent, GraphBasedPlanner, kw, budget, gamma)
+        return lambda m: GBOPDEngine(m, A, budget, gamma, mdp, c["accuracy"], c["sampling_timeout"], device=dev)
+    if planner == "brue":
+        from rl_agents_b200.agents.tree_search.brue import BRUE, BRUEAgent
+        from rl_agents_b200.engine.brue import BRUEEngine
+        c = _completed_config(BRUEAgent, BRUE, kw, budget, gamma)
+        horizon = c["horizon"] if "horizon" in c else allocation(max(A, budget), gamma)[1]
+        return lambda m: BRUEEngine(E, m, A, budget, horizon, gamma, mdp=mdp, device=dev)
+    if planner == "mcts":
+        from rl_agents_b200.engine.mcts import MCTSEngine
+        c = _completed_config(MCTSAgent, MCTS, kw, budget, gamma)
+        episodes, horizon = (c["episodes"], c["horizon"]) if c["horizon"] else allocation(budget, gamma)
+        return lambda m: MCTSEngine(E, m, A, episodes, horizon, gamma, c["temperature"], mdp=mdp,
+                                    rollout_policy=MCTSAgent.policy_factory(c["rollout_policy"]),
+                                    prior_policy=MCTSAgent.policy_factory(c["prior_policy"]), device=dev)
+    if planner == "olop":
+        from rl_agents_b200.agents.tree_search.olop import OLOP, OLOPAgent
+        from rl_agents_b200.engine.olop import OLOPEngine
+        c = _completed_config(OLOPAgent, OLOP, kw, budget, gamma)
+        episodes, horizon = (c["episodes"], c["horizon"]) if "horizon" in c else allocation(max(A, budget), gamma)
+        return lambda m: OLOPEngine(E, m, A, episodes, horizon, gamma, c["upper_bound"], c["continuation_type"],
+                                    mdp=mdp, device=dev)
+    if planner == "mdp_gape":
+        from rl_agents_b200.agents.tree_search.mdp_gape import MDPGapE, MDPGapEAgent, budget_allocation
+        from rl_agents_b200.engine.mdp_gape import MDPGapEEngine
+        c = _completed_config(MDPGapEAgent, MDPGapE, kw, budget, gamma)
+        episodes, horizon = (c["episodes"], c["horizon"]) if "horizon" in c else budget_allocation(c, A)
+        return lambda m: MDPGapEEngine(E, m, A, episodes, horizon, gamma, c["upper_bound"], c["accuracy"],
+                                       c["confidence"], c["continuation_type"], c["max_next_states_count"], mdp=mdp,
+                                       device=dev)
+    if planner == "sparse_sampling":
+        from rl_agents_b200.engine.sparse_sampling import EMPTY_ROOT_MESSAGE, SparseSamplingEngine
+        if kw["horizon"] == 0:
+            raise ValueError(EMPTY_ROOT_MESSAGE)            # SparseSampling.plan: a childless root
+        return lambda m: SparseSamplingEngine(E, m, A, kw["horizon"], kw["C"], gamma, mdp=mdp, device=dev)
+    if planner == "mcts_dpw":
+        from rl_agents_b200.agents.tree_search.mcts_dpw import MCTSDPW, MCTSDPWAgent
+        from rl_agents_b200.engine.mcts_dpw import MCTSDPWEngine
+        c = _completed_config(MCTSDPWAgent, MCTSDPW, kw, budget, gamma)
+        episodes, horizon = (c["episodes"], c["horizon"]) if c["horizon"] else allocation(budget, gamma)
+        return lambda m: MCTSDPWEngine(E, m, A, episodes, horizon, gamma, c["temperature"], c["k_action"],
+                                       c["alpha_action"], c["k_state"], c["alpha_state"], closed_loop=c["closed_loop"],
+                                       rollout_policy=MCTSDPWAgent.policy_factory(c["rollout_policy"]), mdp=mdp,
+                                       device=dev)
+    if planner == "platypoos":
+        from rl_agents_b200.agents.tree_search.platypoos import PlaTyPOOS, PlaTyPOOSAgent
+        from rl_agents_b200.engine.platypoos import PlaTyPOOSEngine, check_plannable, horizon_of
+        c = _completed_config(PlaTyPOOSAgent, PlaTyPOOS, kw, budget, gamma)
+        horizon = c["horizon"] if "horizon" in c else horizon_of(budget, A)
+        check_plannable(horizon, A, True)
+        return lambda m: PlaTyPOOSEngine(E, m, A, horizon, gamma, mdp=mdp, device=dev)
+    raise ValueError("unknown planner %r" % planner)
+
+
+def run_finite_episodes(planner, n_episodes, budget, gamma, mdp, start_states=None, env_seed=0, max_steps=40,
+                        device="cuda", planner_seed=0, **kw):
+    """Closed-loop episodes on a finite MDP in any mode, in lock step: per decision step ONE batched plan() over the
+    live episodes and ONE b2_finite_step over all of them (FiniteMDPEnv.step on the device).
+
+    mdp: a FiniteMDPEnv, or any env adapters.describe takes for a finite MDP.  Episode i starts at start_states[i]
+    (default: the MDP's `state`); its env generator is np.random.default_rng(env_seed + i), the one
+    FiniteMDPEnv(seed=env_seed + i) holds, and its planner generator that of agent.seed(planner_seed + i).  Each
+    episode plays what its planner's drop-in agent, built with dict(kw, budget=budget, gamma=gamma), would act and
+    ends when done (terminal[state the action is taken in]) or at `max_steps`.
+    planner: "opd", "gbop" (GBOP-T), "gbopd" (GBOP-D) and "brue" on deterministic MDPs (NotImplementedError otherwise,
+    as their agents refuse); "mcts", "olop", "mdp_gape", "sparse_sampling", "mcts_dpw" and "platypoos" in every mode;
+    "vi" (ValueIterationAgent, `budget` = its `iterations`).  A reached row that Generator.choice rejects raises its
+    ValueError.
+    Returns dict(returns, lengths, crashed (all False), actions and rewards [n_episodes, steps] (-1 and 0 once an
+    episode has ended), final_states, planner_words and env_words (PCG64 words [n_episodes, 6] at the end),
+    decision_ms (host time per plan step), step_ms (device time per b2_finite_step call), n)."""
+    import torch
+    from rl_agents_b200.engine.mcts import pcg64_words, set_pcg64_words
+    from rl_agents_b200.engine.tables import SampledFiniteTables
+    from rl_agents_b200.envs.adapters import describe
+    d = describe(mdp)
+    if d.kind != _lib.ENV_FINITE:
+        raise ValueError("env 'finite' needs a finite-MDP env (got %r)" % type(mdp).__name__)
+    if planner in DETERMINISTIC_ONLY_PLANNERS and d.mdp.mode != "deterministic":
+        raise NotImplementedError("%r plans on deterministic finite MDPs only (got mode %r)" % (planner, d.mdp.mode))
+    lib = _lib.load()
+    dev = torch.device(device)
+    n, A = int(n_episodes), d.n_actions
+    start = np.full(n, d.root[0]) if start_states is None else np.asarray(start_states)
+    if start.shape != (n,) or (start < 0).any() or (start >= d.mdp.reward.shape[0]).any():
+        raise ValueError("start_states must hold one state id of the MDP per episode")
+    if planner == "vi":
+        from rl_agents_b200.engine.vi import VIEngine
+        m = d.mdp
+        q = VIEngine(m.mode, m.transition, m.reward, m.terminal, nxt=getattr(m, "next", None), gamma=gamma,
+                     device=dev).solve(budget)[0].cpu().numpy()
+    else:
+        make = _finite_engine_factory(planner, d.mdp, A, budget, gamma, kw, dev)
+    tables = SampledFiniteTables(d.mdp, dev)
+    states = torch.as_tensor(start.astype(np.int32), device=dev)
+    env_rng = torch.as_tensor(np.stack([pcg64_words(np.random.default_rng(env_seed + i)) for i in range(n)])
+                              .view(np.int64), device=dev)
+    rngs = [_np_random(planner_seed + i) for i in range(n)]
+    rew = torch.empty(n, dtype=torch.float64, device=dev)
+    flg = torch.empty(n, dtype=torch.int32, device=dev)
+    bad = torch.empty(n, dtype=torch.int32, device=dev)
+    returns, lengths, alive = np.zeros(n), np.zeros(n, dtype=int), np.ones(n, dtype=bool)
+    actions, rewards = np.full((n, max_steps), -1), np.zeros((n, max_steps))
+    eng, events, t_plan, steps = None, [], 0.0, 0
+    for step in range(max_steps):
+        live = np.nonzero(alive)[0]
+        if not live.size:
+            break
+        t0 = time.perf_counter()
+        if planner == "vi":
+            act_live = np.argmax(q[states.cpu().numpy()[live]], axis=1)       # ValueIterationAgent.act
+        else:
+            if eng is None or eng.n_trees != live.size:     # an engine per live-episode count
+                eng = make(live.size)
+            live_d = torch.as_tensor(live, device=dev)
+            roots = states.index_select(0, live_d).contiguous()
+            if planner in ("opd", "gbop"):
+                eng.plan(roots)
+                plans, _ = eng.finish([rngs[i] for i in live])
+            else:
+                words = np.stack([pcg64_words(rngs[i]) for i in live])
+                if planner == "mcts" and eng.sampled:       # MCTSAgent.plan: the live env generator's words
+                    eng.plan(roots, words, None, env_rng.index_select(0, live_d).cpu().numpy().view(np.uint64))
+                else:
+                    eng.plan(roots, words)
+                plans, _, words = eng.finish()
+                for i, w in zip(live, words):
+                    set_pcg64_words(rngs[i], w)
+            act_live = [p[0] for p in plans]
+        t_plan += time.perf_counter() - t0
+        act = np.zeros(n, dtype=np.int32)
+        act[live] = act_live
+        mask = np.zeros(n, dtype=np.uint8)
+        mask[live] = 1
+        act_d, mask_d = torch.from_numpy(act).to(dev), torch.from_numpy(mask).to(dev)
+        events.append((torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)))
+        events[-1][0].record()
+        _lib.check(lib.b2_finite_step(tables.struct(), _lib.ptr(tables.terminal), tables.env_draws, _lib.ptr(states),
+                                      _lib.ptr(act_d), _lib.ptr(mask_d), _lib.ptr(env_rng), _lib.ptr(rew),
+                                      _lib.ptr(flg), _lib.ptr(bad), n, _lib.current_stream()))
+        events[-1][1].record()
+        r, f, b = rew.cpu().numpy(), flg.cpu().numpy(), bad.cpu().numpy()
+        rejected = live[b[live] >= 0]
+        if rejected.size:
+            tables.raise_rejected_row(int(b[rejected[0]]))
+        returns[live] += r[live]
+        rewards[live, step] = r[live]
+        actions[live, step] = act[live]
+        lengths[live] += 1
+        alive[live] = (f[live] & 1) == 0
+        steps += 1
+    step_ms = sum(a.elapsed_time(b) for a, b in events)
+    return {"returns": returns, "lengths": lengths, "crashed": np.zeros(n, dtype=bool), "actions": actions[:, :steps],
+            "rewards": rewards[:, :steps], "final_states": states.cpu().numpy(),
+            "planner_words": np.stack([pcg64_words(g) for g in rngs]), "env_words": env_rng.cpu().numpy().view(np.uint64),
+            "decision_ms": 1e3 * t_plan / max(steps, 1), "step_ms": step_ms / max(steps, 1), "n": n}
