@@ -18,12 +18,15 @@ def main():
     ap.add_argument("--episodes", type=int, default=256)
     ap.add_argument("--gamma", type=float, default=0.8)
     ap.add_argument("--steps", type=int, default=40)
+    ap.add_argument("--step-strategy", default="reset",
+                    help='"subtree": MCTS keeps the sub-tree under the played action (the other planners reset)')
     a = ap.parse_args()
     from rl_agents_b200.evaluation import run_batched_episodes
     print("planner,budget,episodes,mean_return,crash_rate,mean_length,ms_per_batched_decision")
     for planner in a.planners.split(","):
         for budget in [int(b) for b in a.budgets.split(",")]:
-            out = run_batched_episodes(planner, list(range(a.episodes)), budget, a.gamma, max_steps=a.steps)
+            out = run_batched_episodes(planner, list(range(a.episodes)), budget, a.gamma, max_steps=a.steps,
+                                       step_strategy=a.step_strategy)
             print("%s,%d,%d,%.4f,%.4f,%.2f,%.2f" % (planner, budget, a.episodes, out["returns"].mean(),
                                                     out["crashed"].mean(), out["lengths"].mean(), out["decision_ms"]))
             sys.stdout.flush()

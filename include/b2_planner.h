@@ -494,6 +494,25 @@ int b2_mcts_plan_sampled(const b2_mcts_config* cfg, const struct b2_finite_mdp_s
                          int32_t env_draws, const uint64_t* env_rng, const int32_t* root_states,
                          const b2_mcts_tree* tree, uint64_t* rng, int8_t* plan, int32_t* result, void* stream);
 
+/* step_strategy "subtree" (abstract.py:195-206) for a batch of trees, out of place: destination tree j receives the
+ * sub-tree of source tree s = src_tree[j] (src_tree NULL: s = j) under that tree's root child of action action[j],
+ * re-indexed breadth first with the children of a node contiguous and in order; parent / first_child are remapped,
+ * count, meta, value and prior copied, and the new root's action byte set to 0xff.  Bit for bit
+ * engine/mcts.py::reroot_arrays.  One launch can also gather trees into a smaller arena.
+ * src / dst: arenas of [n_src, src_capacity] and [n_dst, dst_capacity] nodes; they must not share an array.
+ * src_nodes[s * src_nodes_stride]: the node count of source tree s (word 0 of the last b2_mcts_plan result, stride
+ * B2_MCTS_RESULT_WORDS).  kept: int32 [n_dst], the nodes written -- resume_nodes for the next b2_mcts_plan, which
+ * then needs dst_capacity >= kept + episodes * n_actions:
+ *   0  when action[j] < 0, when the root has no child of that action, or when kept + reserve > dst_capacity (the
+ *      caller starts a new tree; destination tree j may have been partly written);
+ *  -1  when s is outside [0, n_src) or its node count outside [1, src_capacity] (destination tree j untouched), or
+ *      when a child range of the source leaves [1, node count).
+ * Refused (B2_ERR_INVALID, nothing launched): a null pointer (src_tree excepted), n_dst < 1, n_src, a capacity or
+ * src_nodes_stride < 1, arenas sharing an array, reserve < 0. */
+int b2_mcts_reroot(const b2_mcts_tree* src, int32_t n_src, int32_t src_capacity, const int32_t* src_nodes,
+                   int32_t src_nodes_stride, const b2_mcts_tree* dst, int32_t n_dst, int32_t dst_capacity,
+                   const int32_t* src_tree, const int32_t* action, int32_t reserve, int32_t* kept, void* stream);
+
 /* ------------------------------------------------------------------------
  * Wavefront MCTS: ONE decision searched by the whole GPU.  The reference's episode (selection mcts.py:141-149,
  * expansion :151-154, rollout :160-177, backup :257-265, recommendation :212-218) run in waves of `width`

@@ -264,6 +264,8 @@ EXPORTS = {
                              c_void_p, c_void_p]),
     "b2_mcts_plan_sampled": (c_int, [ctypes.POINTER(MCTSConfig), ctypes.POINTER(FiniteMDPSampled), c_void_p, c_int32,
                                      c_void_p, c_void_p, ctypes.POINTER(MCTSTree)] + [c_void_p] * 4),
+    "b2_mcts_reroot": (c_int, [ctypes.POINTER(MCTSTree), c_int32, c_int32, c_void_p, c_int32, ctypes.POINTER(MCTSTree),
+                               c_int32, c_int32, c_void_p, c_void_p, c_int32, c_void_p, c_void_p]),
     "b2_mcts_wave_workspace_bytes": (c_int64, [ctypes.POINTER(MCTSWaveConfig)]),
     "b2_mcts_plan_wave": (c_int, [ctypes.POINTER(MCTSWaveConfig), c_void_p, ctypes.POINTER(MCTSWaveTree), c_void_p,
                                   c_void_p, c_void_p, c_void_p]),

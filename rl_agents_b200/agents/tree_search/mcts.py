@@ -24,6 +24,12 @@ def allocation(budget, gamma):
     return episodes, horizon
 
 
+def subtree_capacity(episodes, horizon, n_actions):
+    """Nodes per tree under step_strategy "subtree": a node at depth d survives d re-rootings, so a tree holds up to
+    horizon + 1 searches' expansions."""
+    return 1 + (horizon + 1) * episodes * n_actions
+
+
 class MCTS(AbstractPlanner):
     def __init__(self, env, prior_policy, rollout_policy, config=None):
         super(MCTS, self).__init__(config)
@@ -53,10 +59,9 @@ class MCTS(AbstractPlanner):
                self.config["temperature"], repr(self.rollout_policy), repr(self.prior_policy), mdp_fingerprint(d.mdp))
 
         def make():
-            # "subtree" keeps nodes alive for up to `horizon` decisions (a node at depth d survives d re-rootings)
             capacity = None
             if self.config["step_strategy"] == "subtree":
-                capacity = 1 + (self.config["horizon"] + 1) * episodes * d.n_actions
+                capacity = subtree_capacity(episodes, self.config["horizon"], d.n_actions)
             engine = MCTSEngine(d.kind, replicas, d.n_actions, episodes, self.config["horizon"],
                                 self.config["gamma"], self.config["temperature"], mdp=d.mdp,
                                 rollout_policy=self.rollout_policy, prior_policy=self.prior_policy,
@@ -75,8 +80,8 @@ class MCTS(AbstractPlanner):
         if self.config["step_strategy"] == "subtree":
             if actions and self.engine is not None and int(self.config.get("root_parallel", 1) or 1) <= 1 \
                     and self.last_tree is self.engine:
-                self._resume = self.engine.reroot(0, actions[0])          # step_by_subtree (:195-206)
-                if self._resume == 0:
+                self._resume = int(self.engine.reroot([actions[0]])[0])   # step_by_subtree (:195-206)
+                if self._resume <= 0:
                     self.step_by_reset()
             else:
                 self.step_by_reset()

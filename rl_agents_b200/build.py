@@ -8,7 +8,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(CSRC, "libb2planner.so")
 STAMP = LIB + ".cmd"          # signature() of the build that made the library
-SOURCES = ["common.cu", "vi.cu", "vi_p2p.cu", "opd.cu", "opd_wave.cu", "gbop.cu", "mcts.cu", "mcts_wave.cu", "olop.cu",
+SOURCES = ["common.cu", "vi.cu", "vi_p2p.cu", "opd.cu", "opd_wave.cu", "gbop.cu", "mcts.cu", "mcts_reroot.cu", "mcts_wave.cu",
+           "olop.cu",
            "mdp_gape.cu", "brue.cu", "sparse_sampling.cu", "sparse_sampling_levels.cu",
            "mcts_dpw.cu", "platypoos.cu", "ttc_vi.cu", "finite_step.cu", "selftest.cu", "host_api.cu"]
 NVCC_FLAGS = [

@@ -47,7 +47,8 @@ def reroot_arrays(arrays, n, action):
     """step_by_subtree (abstract.py:195-206): keep the sub-tree under the root's child `action`, re-indexed
     breadth first (children of a node stay contiguous and in order) with that child as node 0.
     arrays: dict of numpy arrays parent / first_child / count / meta / value / prior (first n entries valid).
-    Returns (new arrays dict, number of kept nodes) -- (None, 0) when the action was never expanded."""
+    Returns (new arrays dict, number of kept nodes) -- (None, 0) when the action was never expanded.
+    The specification of the device re-root b2_mcts_reroot (MCTSEngine.reroot)."""
     fc, meta = arrays["first_child"], arrays["meta"]
     root_child = -1
     if fc[0] >= 0:
@@ -95,6 +96,7 @@ class MCTSEngine(TreeEngine):
         if self.sampled:
             self.env_rng = torch.empty((self.n_trees, _lib.PCG64_STATE_WORDS), dtype=torch.int64, device=self.device)
         self.tree = _lib.MCTSTree(*self._alloc_tree(_lib.MCTS_TREE_FIELDS, self.capacity))
+        self._spare = None      # reroot's second arena
         self.pref_prior = torch.as_tensor(preference_tables(self.n_actions, prior_ratio)[0], device=self.device)
         self.pref_cdf = torch.as_tensor(preference_tables(self.n_actions, rollout_ratio)[1], device=self.device)
         self.cfg = _lib.MCTSConfig(env_kind, self.n_trees, self.n_actions, self.episodes, self.horizon, self.capacity,
@@ -139,18 +141,42 @@ class MCTSEngine(TreeEngine):
         plans = self.plan_buf.cpu().numpy()
         return [plans[i, :res[i, 1]].astype(int).tolist() for i in range(self.n_trees)]
 
-    def reroot(self, tree, action):
-        """Keep the sub-tree under root child `action` of `tree` (host-side compaction, once per decision).
-        Returns the number of nodes kept (0: the action was never expanded -> start a new tree)."""
-        n = int(self.result[tree, 0].item())
-        names = _lib.MCTS_TREE_FIELDS
-        arrays = {k: getattr(self, k)[tree, :n].cpu().numpy() for k in names}
-        out, kept = reroot_arrays(arrays, n, int(action))
-        if kept + self.episodes * self.n_actions > self.capacity:
-            return 0                                   # would not fit: fall back to a fresh tree
-        for k in names if kept else ():
-            getattr(self, k)[tree, :kept] = self.torch.as_tensor(out[k], device=self.device)
-        return kept
+    def _arena(self):
+        return tuple(getattr(self, k) for k in _lib.MCTS_TREE_FIELDS)
+
+    def _use_arena(self, arena):
+        for k, t in zip(_lib.MCTS_TREE_FIELDS, arena):
+            setattr(self, k, t)
+        self.tree = _lib.MCTSTree(*[t.data_ptr() for t in arena])
+
+    def reroot(self, actions, sources=None, source=None):
+        """step_strategy "subtree" for every tree in one launch (b2_mcts_reroot): tree j becomes the sub-tree of tree
+        sources[j] (default j) of `source` (default this engine), as its last plan left it, under that tree's root
+        child of action actions[j] -- reroot_arrays, on the device.  Re-rooting within this engine writes a spare
+        arena, allocated on first use, and swaps it in; from another engine (the survivors of a batch gathered into a
+        smaller one) it writes this engine's arena.
+        -> kept, int32 numpy [n_trees]: the node counts to pass as plan(resume_nodes=...); 0 starts a new tree (the
+        action is < 0 or was never expanded, or the sub-tree and this engine's episodes * n_actions new nodes would
+        not fit), -1 reports a source index outside `source`'s trees."""
+        torch = self.torch
+        src = self if source is None else source
+        if src is self:
+            if self._spare is None:
+                self._spare = tuple(torch.empty_like(t) for t in self._arena())
+            dst = _lib.MCTSTree(*[t.data_ptr() for t in self._spare])
+        else:
+            dst = self.tree
+        act = torch.as_tensor(np.asarray(actions, dtype=np.int32).reshape(self.n_trees), device=self.device)
+        idx = None if sources is None else \
+            torch.as_tensor(np.asarray(sources, dtype=np.int32).reshape(self.n_trees), device=self.device)
+        _lib.check(self.lib.b2_mcts_reroot(src.tree, src.n_trees, src.capacity, _lib.ptr(src.result),
+                                           _lib.MCTS_RESULT_WORDS, dst, self.n_trees, self.capacity, _lib.ptr(idx),
+                                           _lib.ptr(act), self.episodes * self.n_actions, _lib.ptr(self.resume),
+                                           _lib.current_stream()))
+        if src is self:
+            spare, self._spare = self._spare, self._arena()
+            self._use_arena(spare)
+        return self.resume.cpu().numpy()
 
     def tree_dict(self, tree=0):
         n = int(self.result[tree, 0].item())

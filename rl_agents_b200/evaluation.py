@@ -3,12 +3,15 @@ planner on finite MDPs, stepped by b2_finite_step): the
 working version of the reference's disabled budget-sweep harness (scripts/planners_evaluation.py:287-289, SURVEY 8f
 rank 4) in the shape the GPU wants -- all episodes advance in lock-step, every decision step is
 ONE batched plan() launch over all live episodes and ONE batched env transition."""
+import logging
 import time
 
 import numpy as np
 
 from rl_agents_b200 import _lib
 from rl_agents_b200.envs import highway_lite, intersection_lite
+
+logger = logging.getLogger(__name__)
 
 # planners with an IntersectionLite model (b2_mcts_plan, b2_olop_plan)
 INTERSECTION_PLANNERS = ("mcts", "olop")
@@ -22,6 +25,18 @@ def _np_random(seed):
     return np.random.Generator(np.random.PCG64(np.random.SeedSequence(seed)))
 
 
+def _keeps_subtrees(planner, kw):
+    """Whether the episodes of `planner` keep their trees across decisions: keyword step_strategy "subtree" on "mcts",
+    as MCTSAgent does.  Any other strategy than "reset" resets, with the warning the agents give."""
+    strategy = kw.get("step_strategy", "reset")
+    if planner == "mcts" and strategy == "subtree":
+        return True
+    if strategy != "reset":
+        logger.warning("step strategy {} is not supported by the batched {} episodes: resetting".format(strategy,
+                                                                                                        planner))
+    return False
+
+
 def run_batched_episodes(planner, seeds, budget, gamma, max_steps=40, device="cuda", planner_seed=0, env="highway",
                          **kw):
     """planner: "opd" | "mcts" | "olop" | "mdp_gape" (keywords: MDPGapEAgent config keys) | "brue" (keywords: BRUEAgent
@@ -29,13 +44,16 @@ def run_batched_episodes(planner, seeds, budget, gamma, max_steps=40, device="cu
     is unused) | "mcts_dpw" (keywords: MCTSDPWAgent config keys) | "platypoos" (keywords: PlaTyPOOSAgent config keys;
     the first action of each plan is played) | "vi" (ValueIterationAgent on the scenes' TTC-grid MDPs, `budget` = its
     `iterations`).  Every episode: scene make_scene(seed), replanning at every step (receding_horizon 1, step_strategy reset -- the reference
-    defaults), until crash or `max_steps`.
+    defaults), until crash or `max_steps`.  "mcts" also takes step_strategy="subtree" (on every env): after each step
+    every tree is re-rooted at its played action in one b2_mcts_reroot launch and the next search resumes from it, so
+    episode i plays what MCTSAgent(env_i, {budget, gamma, step_strategy: "subtree"}) seeded planner_seed + i plays.
     env: "highway" (HighwayLite, every planner) or "intersection" (IntersectionLite scenes of
     envs.intersection_lite.make_scene stepped by b2_intersection_step, "mcts" and "olop" only; an episode also ends
     when the ego arrives or at the env's duration).  `crashed` is the ego's crash flag.
     env "finite": closed-loop episodes on a finite MDP, see run_finite_episodes (keywords `mdp`, `start_states`,
     `env_seed`).
-    Returns dict(returns, lengths, crashed, decision_ms)."""
+    Returns dict(returns, lengths, crashed, decision_ms), with "subtree" also `resumed`: per episode, the decisions
+    that resumed a kept sub-tree."""
     if env == "finite":
         return run_finite_episodes(planner, len(seeds), budget, gamma, max_steps=max_steps, device=device,
                                    planner_seed=planner_seed, **kw)
@@ -45,7 +63,7 @@ def run_batched_episodes(planner, seeds, budget, gamma, max_steps=40, device="cu
     from rl_agents_b200.engine.mcts import MCTSEngine, pcg64_words, set_pcg64_words
     from rl_agents_b200.engine.olop import OLOPEngine
     from rl_agents_b200.engine.opd import OPDEngine
-    from rl_agents_b200.agents.tree_search.mcts import allocation
+    from rl_agents_b200.agents.tree_search.mcts import allocation, subtree_capacity
     if env == "highway":
         env_kind, n_actions, make_scene = _lib.ENV_HIGHWAY, 5, highway_lite.make_scene
     elif env == "intersection":
@@ -55,6 +73,7 @@ def run_batched_episodes(planner, seeds, budget, gamma, max_steps=40, device="cu
         env_kind, n_actions, make_scene = _lib.ENV_INTERSECTION, intersection_lite.N_ACTIONS, intersection_lite.make_scene
     else:
         raise ValueError("unknown env %r" % env)
+    subtree = _keeps_subtrees(planner, kw)
     lib = _lib.load()
     dev = torch.device(device)
     n = len(seeds)
@@ -67,7 +86,8 @@ def run_batched_episodes(planner, seeds, budget, gamma, max_steps=40, device="cu
         from rl_agents_b200.agents.tree_search.mcts import MCTS
         # the reference's default temperature comes from the CLASS default gamma (mcts.py:120-127), not the configured one
         eng = MCTSEngine(env_kind, n, n_actions, episodes, horizon, gamma,
-                         kw.get("temperature", MCTS.default_config()["temperature"]), device=dev)
+                         kw.get("temperature", MCTS.default_config()["temperature"]), device=dev,
+                         capacity=subtree_capacity(episodes, horizon, n_actions) if subtree else None)
     elif planner == "olop":
         episodes, horizon = allocation(max(n_actions, budget), gamma)
         ub = kw.get("upper_bound", {"type": "kullback-leibler", "time": "global", "threshold": "2*np.log(time)"})
@@ -127,17 +147,26 @@ def run_batched_episodes(planner, seeds, budget, gamma, max_steps=40, device="cu
     flg = torch.empty(n, dtype=torch.int32, device=dev)
     actions_log = []
     t_plan = 0.0
+    kept, resumed = None, np.zeros(n, dtype=int)
     for step in range(max_steps):
         if not alive.any():
             break
         t0 = time.perf_counter()
+        if subtree and step:
+            # MCTS.step_tree: every tree re-rooted at its played action (-1 after an empty plan: a new tree)
+            kept = eng.reroot([p[0] if p else -1 for p in plans])
+            resumed += alive & (kept > 0)
         if planner == "opd":
             eng.plan(scenes)
             plans, _ = eng.finish(rngs)
         elif planner == "vi":
             plans = [[int(a)] for a in eng.solve(scenes, want_q=False)["action"].cpu().numpy()]
         else:
-            eng.plan(scenes, np.stack([pcg64_words(g) for g in rngs]))
+            words = np.stack([pcg64_words(g) for g in rngs])
+            if kept is None:
+                eng.plan(scenes, words)
+            else:
+                eng.plan(scenes, words, kept)
             plans, _, words = eng.finish()
             for g, w in zip(rngs, words):
                 set_pcg64_words(g, w)
@@ -156,8 +185,11 @@ def run_batched_episodes(planner, seeds, budget, gamma, max_steps=40, device="cu
         else:       # IntersectionLite also terminates on arrival: the crash is bit 1 of the ego's flags word
             crashed |= alive & ((scenes[:, 48].cpu().numpy() & 2) != 0)
         alive &= ~done
-    return {"returns": returns, "lengths": lengths, "crashed": crashed, "actions": np.array(actions_log).T,
-            "decision_ms": 1e3 * t_plan / max(len(actions_log), 1), "n": n}
+    out = {"returns": returns, "lengths": lengths, "crashed": crashed, "actions": np.array(actions_log).T,
+           "decision_ms": 1e3 * t_plan / max(len(actions_log), 1), "n": n}
+    if subtree:
+        out["resumed"] = resumed        # per episode: the decisions that resumed a kept sub-tree
+    return out
 
 
 def _completed_config(agent_cls, planner_cls, kw, budget, gamma):
@@ -199,12 +231,15 @@ def _finite_engine_factory(planner, mdp, n_actions, budget, gamma, kw, dev):
         horizon = c["horizon"] if "horizon" in c else allocation(max(A, budget), gamma)[1]
         return lambda m: BRUEEngine(E, m, A, budget, horizon, gamma, mdp=mdp, device=dev)
     if planner == "mcts":
+        from rl_agents_b200.agents.tree_search.mcts import subtree_capacity
         from rl_agents_b200.engine.mcts import MCTSEngine
         c = _completed_config(MCTSAgent, MCTS, kw, budget, gamma)
         episodes, horizon = (c["episodes"], c["horizon"]) if c["horizon"] else allocation(budget, gamma)
+        capacity = subtree_capacity(episodes, horizon, A) if c["step_strategy"] == "subtree" else None
         return lambda m: MCTSEngine(E, m, A, episodes, horizon, gamma, c["temperature"], mdp=mdp,
                                     rollout_policy=MCTSAgent.policy_factory(c["rollout_policy"]),
-                                    prior_policy=MCTSAgent.policy_factory(c["prior_policy"]), device=dev)
+                                    prior_policy=MCTSAgent.policy_factory(c["prior_policy"]), device=dev,
+                                    capacity=capacity)
     if planner == "olop":
         from rl_agents_b200.agents.tree_search.olop import OLOP, OLOPAgent
         from rl_agents_b200.engine.olop import OLOPEngine
@@ -253,7 +288,9 @@ def run_finite_episodes(planner, n_episodes, budget, gamma, mdp, start_states=No
     (default: the MDP's `state`); its env generator is np.random.default_rng(env_seed + i), the one
     FiniteMDPEnv(seed=env_seed + i) holds, and its planner generator that of agent.seed(planner_seed + i).  Each
     episode plays what its planner's drop-in agent, built with dict(kw, budget=budget, gamma=gamma), would act and
-    ends when done (terminal[state the action is taken in]) or at `max_steps`.
+    ends when done (terminal[state the action is taken in]) or at `max_steps`.  With "mcts" and step_strategy="subtree"
+    every live tree is re-rooted at its played action after each step (b2_mcts_reroot), into a new engine holding the
+    survivors' trees only when episodes have ended, and the next search resumes from it.
     planner: "opd", "gbop" (GBOP-T), "gbopd" (GBOP-D) and "brue" on deterministic MDPs (NotImplementedError otherwise,
     as their agents refuse); "mcts", "olop", "mdp_gape", "sparse_sampling", "mcts_dpw" and "platypoos" in every mode;
     "vi" (ValueIterationAgent, `budget` = its `iterations`).  A reached row that Generator.choice rejects raises its
@@ -270,6 +307,7 @@ def run_finite_episodes(planner, n_episodes, budget, gamma, mdp, start_states=No
         raise ValueError("env 'finite' needs a finite-MDP env (got %r)" % type(mdp).__name__)
     if planner in DETERMINISTIC_ONLY_PLANNERS and d.mdp.mode != "deterministic":
         raise NotImplementedError("%r plans on deterministic finite MDPs only (got mode %r)" % (planner, d.mdp.mode))
+    subtree = _keeps_subtrees(planner, kw)
     lib = _lib.load()
     dev = torch.device(device)
     n, A = int(n_episodes), d.n_actions
@@ -294,6 +332,7 @@ def run_finite_episodes(planner, n_episodes, budget, gamma, mdp, start_states=No
     returns, lengths, alive = np.zeros(n), np.zeros(n, dtype=int), np.ones(n, dtype=bool)
     actions, rewards = np.full((n, max_steps), -1), np.zeros((n, max_steps))
     eng, events, t_plan, steps = None, [], 0.0, 0
+    planned, kept, resumed = None, None, np.zeros(n, dtype=int)     # "subtree": the episodes of the last plan
     for step in range(max_steps):
         live = np.nonzero(alive)[0]
         if not live.size:
@@ -303,7 +342,15 @@ def run_finite_episodes(planner, n_episodes, budget, gamma, mdp, start_states=No
             act_live = np.argmax(q[states.cpu().numpy()[live]], axis=1)       # ValueIterationAgent.act
         else:
             if eng is None or eng.n_trees != live.size:     # an engine per live-episode count
-                eng = make(live.size)
+                old, eng = eng, make(live.size)
+                if subtree and old is not None:             # the survivors' trees, gathered and re-rooted
+                    kept = eng.reroot(act[live], np.searchsorted(planned, live), source=old)
+                del old
+            elif subtree and planned is not None:           # MCTS.step_tree, every tree in one launch
+                kept = eng.reroot(act[live])
+            if kept is not None:
+                resumed[live] += kept > 0
+            planned = live
             live_d = torch.as_tensor(live, device=dev)
             roots = states.index_select(0, live_d).contiguous()
             if planner in ("opd", "gbop"):
@@ -311,8 +358,9 @@ def run_finite_episodes(planner, n_episodes, budget, gamma, mdp, start_states=No
                 plans, _ = eng.finish([rngs[i] for i in live])
             else:
                 words = np.stack([pcg64_words(rngs[i]) for i in live])
-                if planner == "mcts" and eng.sampled:       # MCTSAgent.plan: the live env generator's words
-                    eng.plan(roots, words, None, env_rng.index_select(0, live_d).cpu().numpy().view(np.uint64))
+                if planner == "mcts":       # MCTSAgent.plan: the resumed sub-trees and the live env generator's words
+                    eng.plan(roots, words, kept,
+                             env_rng.index_select(0, live_d).cpu().numpy().view(np.uint64) if eng.sampled else None)
                 else:
                     eng.plan(roots, words)
                 plans, _, words = eng.finish()
@@ -342,7 +390,10 @@ def run_finite_episodes(planner, n_episodes, budget, gamma, mdp, start_states=No
         alive[live] = (f[live] & 1) == 0
         steps += 1
     step_ms = sum(a.elapsed_time(b) for a, b in events)
-    return {"returns": returns, "lengths": lengths, "crashed": np.zeros(n, dtype=bool), "actions": actions[:, :steps],
-            "rewards": rewards[:, :steps], "final_states": states.cpu().numpy(),
-            "planner_words": np.stack([pcg64_words(g) for g in rngs]), "env_words": env_rng.cpu().numpy().view(np.uint64),
-            "decision_ms": 1e3 * t_plan / max(steps, 1), "step_ms": step_ms / max(steps, 1), "n": n}
+    out = {"returns": returns, "lengths": lengths, "crashed": np.zeros(n, dtype=bool), "actions": actions[:, :steps],
+           "rewards": rewards[:, :steps], "final_states": states.cpu().numpy(),
+           "planner_words": np.stack([pcg64_words(g) for g in rngs]), "env_words": env_rng.cpu().numpy().view(np.uint64),
+           "decision_ms": 1e3 * t_plan / max(steps, 1), "step_ms": step_ms / max(steps, 1), "n": n}
+    if subtree:
+        out["resumed"] = resumed        # per episode: the decisions that resumed a kept sub-tree
+    return out
